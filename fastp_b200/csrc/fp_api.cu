@@ -933,7 +933,11 @@ static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
     if (want_ev) {
         *c->ev_host_n = 0;
         if (!c->d_ev[0]) {
-            c->ev_chunk_cap = (uint32_t)std::min<int64_t>(CH * 4 + 1024, (int64_t)1 << 24);   /* a unit gives at most 2 events + 2 per fasta adapter */
+            /* a pair gives at most 2 events (trimByOverlapAnalysis, or trimBySequence on each read) + 1 per fasta adapter and read; a read
+               1 + 1 per fasta adapter.  Past 2^24 entries (a full chunk with more than 30 fasta adapters PE, 62 SE) a chunk could still
+               overflow: finish() fails then */
+            const int64_t per_unit = pe ? 2 + 2 * (int64_t)c->p.n_fasta_adapters : 1 + (int64_t)c->p.n_fasta_adapters;
+            c->ev_chunk_cap = (uint32_t)std::min<int64_t>(CH * per_unit + 1024, (int64_t)1 << 24);
             for (int i = 0; i < 2; i++) {
                 CK(cudaMalloc(&c->d_ev[i], (size_t)c->ev_chunk_cap * sizeof(fp_adapter_event))); CK(cudaMalloc(&c->d_nev[i], 4));
                 CK(cudaMallocHost(&c->h_ev[i], (size_t)c->ev_chunk_cap * sizeof(fp_adapter_event))); CK(cudaMallocHost(&c->h_nev[i], 4));
@@ -944,6 +948,8 @@ static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
     fp_adapter_event* const saved_dev = c->ev_dev; const uint32_t saved_cap = c->ev_cap; uint32_t* const saved_cnt = c->ev_count;
     struct Restore { fp_ctx* c; fp_adapter_event* d; uint32_t cap; uint32_t* n; ~Restore() { c->ev_dev = d; c->ev_cap = cap; c->ev_count = n; } } restore{c, saved_dev, saved_cap, saved_cnt};
     if (!want_ev) { c->ev_dev = nullptr; c->ev_cap = 0; c->ev_count = nullptr; }
+    /* a chunk that fails in finish() returns early: leave no copy into the caller's buffers in flight behind the return */
+    struct Drain { fp_ctx* c; ~Drain() { cudaStreamSynchronize(c->stream[0]); cudaStreamSynchronize(c->stream[1]); } } drain{c};
     /* finish(k): host side of chunk k.  Device buffers belong to slot k & 1, the host patch buffers and `pend` to k % 4: the device slot
        is handed to chunk k + 2 as soon as the chunk's event has fired, while its patches are still being written back here. */
     auto finish = [&](int64_t k) -> int {
@@ -953,13 +959,13 @@ static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
                                                                     chunk in flight on the HOST side (k % 4): the slot's next chunk records its own */
         if (want_ev) {
             const uint32_t ne = *c->h_nev[slot];
-            const uint32_t have = std::min(ne, c->ev_chunk_cap);
-            if (have > 0) CK(cudaMemcpy(c->h_ev[slot], c->d_ev[slot], (size_t)have * sizeof(fp_adapter_event), cudaMemcpyDeviceToHost));
-            for (uint32_t i = 0; i < have; i++) {
+            /* the kernel dropped what did not fit: the caller's list would have a hole in the middle */
+            if (ne > c->ev_chunk_cap) return set_err(FP_E_TOOLARGE, "adapter events of one host chunk exceed its event buffer (too many fasta adapters)");
+            if (ne > 0) CK(cudaMemcpy(c->h_ev[slot], c->d_ev[slot], (size_t)ne * sizeof(fp_adapter_event), cudaMemcpyDeviceToHost));
+            for (uint32_t i = 0; i < ne; i++) {
                 if (*c->ev_host_n < c->ev_host_cap) { c->ev_host[*c->ev_host_n] = c->h_ev[slot][i]; c->ev_host[*c->ev_host_n].unit = (uint32_t)(pend[hs].lo + c->h_ev[slot][i].unit); }
                 (*c->ev_host_n)++;
             }
-            if (ne > have) *c->ev_host_n += ne - have;           /* more events than the chunk buffer holds: counted, not listed */
         }
         if (pe && c->p.correction_enabled) {
             uint32_t np = *c->h_npatch[hs];
@@ -995,7 +1001,9 @@ static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
                         (*hp_n)++;
                     }
             } else if (pk) {
-                if (hp_n) *hp_n = ~(uint64_t)0 >> 1;             /* the caller's list cannot be complete */
+                /* packed input: the list is the only way corrections reach the caller, and the kernel did not list all of this chunk's */
+                if (hp_n) return set_err(FP_E_TOOLARGE, "base corrections of one host chunk exceed its patch list: the packed entry point cannot return them "
+                                                        "all (use fp_process_pe_host_patches, which writes the corrected rows back)");
             } else {   /* patch list overflow: take the corrected rows wholesale (row by row when the host pitch differs); the issuing loop
                           keeps the device slot until this is done (it sees the same count) */
                 if (hp_n) *hp_n = ~(uint64_t)0 >> 1;             /* the caller's list cannot be complete */
