@@ -245,6 +245,13 @@ static void make_smem_layout(fp_ctx* c) {
        group barrier, bit 1 = L2 prefetch of the CTA's next tile (off: 1 - 1.5 % faster on every bench workload on an H100) */
     c->sl.xflags = 0;
     if (const char* e = getenv("FP_XFLAGS")) c->sl.xflags = atoi(e);
+    /* threads per column of the dense column pass (phase A's dense_tile, phase C's dense_remove): as many as fit in 5/8 of the group
+       (10 of 16 warps), at least one.  The column pass needs no item and no item needs it, so the warps without columns start the plane /
+       histogram items at once and the column warps join them when their rows are done.  With every thread on columns (3 per column at
+       2 x 150 bp, 2 at 2 x 250 bp) one warp or none started the items early; on an H100 10 column warps were best for PE and SE at stride
+       160 and 8 for PE at stride 256 (DESIGN.md section 9) */
+    const int ncols = sides * (c->stride / 2);
+    c->sl.col_split = std::max(1, c->group_threads * 5 / 8 / ncols);
 }
 
 static int ctx_init(fp_ctx* c, const fp_params* p, int device, int64_t max_batch, int32_t stride, int32_t cycles);
@@ -436,7 +443,7 @@ static int ctx_init(fp_ctx* c, const fp_params* p, int device, int64_t max_batch
     }
     if (occ < 1) return set_err(FP_E_CUDA, "kernel cannot be resident (shared memory / registers)");
     c->grid_max = occ * c->num_sms;
-    if (getenv("FP_TRACE")) fprintf(stderr, "[fastp_b200] groups %d x %d threads, tile %d rows, smem %d B (shared %d + %d per group), %d CTA/SM\n", c->groups, c->group_threads, c->tile, c->sl.total, c->sl.off_group, c->sl.group_stride, occ);
+    if (getenv("FP_TRACE")) fprintf(stderr, "[fastp_b200] groups %d x %d threads, tile %d rows, smem %d B (shared %d + %d per group), %d CTA/SM, %d threads per column\n", c->groups, c->group_threads, c->tile, c->sl.total, c->sl.off_group, c->sl.group_stride, occ, c->sl.col_split);
     return FP_OK;
 }
 

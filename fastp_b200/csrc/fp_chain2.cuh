@@ -1580,9 +1580,9 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
     /* column-pass ownership: thread = (side, half-word column): cycles 2*hc, 2*hc+1 */
     const int HPR = S >> 1;
     const int ncols = SIDES * HPR;                /* host guarantees ncols <= CT */
-    const int nsplit = CT / ncols;             /* row groups are dealt round-robin to nsplit threads per column */
+    const int nsplit = sl.col_split;              /* row groups are dealt round-robin to nsplit threads per column; host: 1 <= nsplit <= CT / ncols */
     const bool col_active = tid < ncols * nsplit;
-    const int my_part = col_active ? tid / ncols : 0, my_col = col_active ? tid % ncols : 0;
+    const int my_part = tid / ncols, my_col = col_active ? tid % ncols : 0;     /* my_part is read by column threads only */
     const int my_side = my_col / HPR, my_hc = my_col % HPR;
     const int my_w = my_hc >> 1, my_half = my_hc & 1;
     ColAcc2 acc;
@@ -1619,7 +1619,7 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
     uint32_t parity = 0;
 #ifdef FP_PHASE_TIMING
     /* measurement build (scripts/gpu_phase_timing.sh): cycles each warp of CTA 0 spends up to every barrier of a tile, summed over the launch */
-    long long tph[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0}, tlast = clock64();
+    long long tph[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0}, tlast = clock64();
 #define FP_TP(k) do { const long long tn_ = clock64(); tph[k] += tn_ - tlast; tlast = tn_; } while (0)
 #else
 #define FP_TP(k) do { } while (0)
@@ -1661,6 +1661,7 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
         /* ---------------- phase A: dense pass (column warps) || bit planes + validation (other warps) ---------------- */
         if (col_active)           /* dense column pass: pre-filter stats of every row of the tile, two cycles per thread */
             dense_tile(acc, tile_seq[my_side], tile_qual[my_side], s_len + my_side * T, rows, S, my_w * 4, my_half, 4 * my_part, 4 * nsplit, G, my_side);
+        FP_TP(10);
         {   /* bit planes + validation: 32-item batches claimed dynamically -- warps without columns start at once, the dense warps join */
             const int nwords = (S + 31) >> 5;
             const uint32_t qq4 = (uint32_t)(c_p.qualified_qual & 0x7F) * 0x01010101u;
@@ -2087,6 +2088,7 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
                 if (nr > 0) dense_remove(s_bk + my_side * NBK * (T + 4), s_nbk + my_side * NBK, NBK, T + 4, my_part, nsplit, tile_seq[my_side], tile_qual[my_side], S, my_w * 4, my_half,
                                          D.cyc + my_side * S * 20, S);
             }
+            FP_TP(11);
             /* (2) qualities and 5-mers of the removal lists: one lane per (entry, 32-base chunk), claimed 32 at a time */
             {
                 const int nwords = (S + 31) >> 5;
@@ -2143,8 +2145,8 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
 
 #ifdef FP_PHASE_TIMING
     if (blockIdx.x == 0 && lane == 0)
-        printf("PHASE warp %2d tma %lld busyA %lld totA %lld busyB1 %lld totB1 %lld corr %lld busyB2 %lld totB2 %lld busyC %lld totC %lld\n", warp,
-               tph[0], tph[1], tph[2], tph[3], tph[4], tph[5], tph[6], tph[7], tph[8], tph[9]);
+        printf("PHASE warp %2d col %d tma %lld colA %lld itemsA %lld totA %lld busyB1 %lld totB1 %lld corr %lld busyB2 %lld totB2 %lld colC %lld itemsC %lld totC %lld\n",
+               warp, col_active ? 1 : 0, tph[0], tph[10], tph[1], tph[2], tph[3], tph[4], tph[5], tph[6], tph[7], tph[11], tph[8], tph[9]);
 #endif
     __syncthreads();                               /* every group is done with the shared tables */
     /* ---------------- flush block-level accumulators ---------------- */

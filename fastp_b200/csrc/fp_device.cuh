@@ -375,7 +375,8 @@ __device__ __noinline__ void dev_stat_positions_smem(const DeltaAcc D, int side,
 struct fp_smem_layout {
     int off_dummy, off_mbar, off_next, off_tile, tile_array_bytes, off_len, off_clean, off_kmer, off_qhist, off_bc, off_lut, off_delta,
         off_dkmer, off_dqh, off_rm, off_planes, off_queue, plane_words, plane_stride, total,
-        off_group, group_stride, off_corr, off_cm, cm_words, xflags;     /* off_mbar, off_next, off_len, off_clean, off_tile, off_rm, off_planes, off_queue are relative to a group's region */
+        off_group, group_stride, off_corr, off_cm, cm_words, xflags,     /* off_mbar, off_next, off_len, off_clean, off_tile, off_rm, off_planes, off_queue are relative to a group's region */
+        col_split;                   /* threads per column of the dense column pass, 1 .. CT / (sides * stride / 2) (fp_api.cu make_smem_layout) */
 };
 
 struct fp_launch_args {
