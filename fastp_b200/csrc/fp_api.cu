@@ -55,8 +55,6 @@ struct fp_ctx {
     fp_counter_layout L{};
     int64_t max_batch = 0;
     int stride = 0, cycles = 0, tile = 0, grid_max = 0, num_sms = 0;
-    int group_threads = 512;            /* one 16-warp group per SM (FP_GROUP_THREADS=256: 8-warp groups, FP_GROUPS of them) */
-    int groups = 1;                     /* tile pipelines per CTA (fp_chain2_kernel<.., NG>) sharing the histogram tables; FP_GROUPS=1|2|3 overrides (3 x 8 warps needs <= 80 registers: measured slower) */
     fp_smem_layout sl{};
     uint32_t smem_base = 1024;        /* shared-window address of dynamic shared memory (probed) */
     cudaStream_t stream[2] = {nullptr, nullptr};
@@ -171,20 +169,11 @@ __global__ void fp_probe_smem_base(uint32_t* out) { extern __shared__ uint8_t pr
 
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-/* kernel shapes: groups x threads per group.  (2, 256) = two 8-warp tile pipelines per CTA, one CTA per SM (the default);
-   (1, 256) = round 1's shape, two CTAs per SM; (3, 256) = 24 warps per SM at <= 80 registers; (1, 512) = ONE 16-warp pipeline per SM
-   with 128-pair tiles: every warp of the SM is in the same phase, i.e. one hot code region at a time (instruction cache). */
-static const void* chain_kernel(bool paired, int groups, int ct) {
-    if (ct == 512) return paired ? (const void*)fp_chain2_kernel<true, 1, 512> : (const void*)fp_chain2_kernel<false, 1, 512>;
-    if (paired) return groups == 1 ? (const void*)fp_chain2_kernel<true, 1, 256> : groups == 2 ? (const void*)fp_chain2_kernel<true, 2, 256> : (const void*)fp_chain2_kernel<true, 3, 256>;
-    return groups == 1 ? (const void*)fp_chain2_kernel<false, 1, 256> : groups == 2 ? (const void*)fp_chain2_kernel<false, 2, 256> : (const void*)fp_chain2_kernel<false, 3, 256>;
-}
-
 static size_t smem_layout_for_tile(fp_ctx* c, int T, fp_smem_layout& sl) {
     const int sides = c->p.paired ? 2 : 1;
     const int S = c->stride;
     memset(&sl, 0, sizeof(sl));
-    /* ---- shared by the CTA's groups: sink, LUTs, histograms, delta accumulators, block counters ---- */
+    /* ---- tables that live for the whole kernel: sink, LUTs, histograms, delta accumulators, block counters ---- */
     size_t off = 0;
     sl.off_dummy = (int)off; off += 128;
     sl.off_lut = (int)off; off += align_up((size_t)3 * (S + 2) * 2, 16);
@@ -199,59 +188,50 @@ static size_t smem_layout_for_tile(fp_ctx* c, int T, fp_smem_layout& sl) {
     sl.off_dqh = (int)off; off += (size_t)sides * FP_QUAL_BINS * 4;
     off = align_up(off, 16);
     sl.off_bc = (int)off; off += sizeof(BlockCounters);
+    /* ---- the tile pipeline: mbarrier, cursors, lengths, tile, planes, removal lists, request queue ---- */
     off = align_up(off, 128);
-    sl.off_group = (int)off;
-    /* ---- one region per group (offsets relative to it): mbarrier, cursors, lengths, tile, planes, removal lists, request queue ---- */
-    size_t g = 0;
-    sl.off_mbar = (int)g; g += 16;
-    sl.off_next = (int)g; g += 32;                                         /* queue length, pop cursor, item cursors, correction list length */
-    sl.off_len = (int)g; g += (size_t)sides * T * 2;
-    sl.off_clean = (int)g; g += (size_t)sides * T;
-    g = align_up(g, 128);
-    sl.off_tile = (int)g; sl.tile_array_bytes = T * S; g += (size_t)sides * 2 * T * S + 32;   /* + slack for 32-byte plane reads */
-    g = align_up(g, 16);
+    sl.off_mbar = (int)off; off += 16;
+    sl.off_next = (int)off; off += 32;                                     /* queue length, pop cursor, item cursors, correction list length */
+    sl.off_len = (int)off; off += (size_t)sides * T * 2;
+    sl.off_clean = (int)off; off += (size_t)sides * T;
+    off = align_up(off, 128);
+    sl.off_tile = (int)off; sl.tile_array_bytes = T * S; off += (size_t)sides * 2 * T * S + 32;   /* + slack for 32-byte plane reads */
+    off = align_up(off, 16);
     {   /* removal lists (one per side, padded to 4 entries) + their lengths (4 words), then the same entries in buckets by lo >> 5
            (per-cycle part of phase C) + their lengths; one region, see DeltaSinks */
         const size_t nbk = (size_t)(S + 31) / 32;
-        sl.off_rm = (int)g; g += (size_t)sides * (T + 4) * 4 + 16 + sides * nbk * (size_t)(T + 4) * 4 + sides * nbk * 4;
+        sl.off_rm = (int)off; off += (size_t)sides * (T + 4) * 4 + 16 + sides * nbk * (size_t)(T + 4) * 4 + sides * nbk * 4;
     }
     sl.plane_words = (S + 31) / 32 + 2;
     sl.plane_stride = (5 * sl.plane_words) | 1;                            /* odd: one lane group per row without bank conflicts */
-    g = align_up(g, 16);
-    sl.off_planes = (int)g; g += (size_t)sides * T * sl.plane_stride * 4;
-    g = align_up(g, 16);
-    sl.off_queue = (int)g; g += (size_t)sides * T * 2 * 8;
+    off = align_up(off, 16);
+    sl.off_planes = (int)off; off += (size_t)sides * T * sl.plane_stride * 4;
+    off = align_up(off, 16);
+    sl.off_queue = (int)off; off += (size_t)sides * T * 2 * 8;
     if (sides == 2) {                                                      /* base correction: work list + per-row masks of corrected positions */
         sl.cm_words = (S + 31) / 32;
-        sl.off_corr = (int)g; g += (size_t)FP_CORR_CAP * 4 + 16;                        /* the tile's list + its length */
-        sl.off_cm = (int)g; g += (size_t)sides * T * sl.cm_words * 4;
+        sl.off_corr = (int)off; off += (size_t)FP_CORR_CAP * 4 + 16;                    /* the tile's list + its length */
+        sl.off_cm = (int)off; off += (size_t)sides * T * sl.cm_words * 4;
     }
-    sl.group_stride = (int)align_up(g, 128);
-    sl.total = (int)align_up(off + (size_t)c->groups * sl.group_stride, 128);
+    sl.total = (int)align_up(off, 128);
     return (size_t)sl.total;
 }
 
-/* tile size: as large as possible (<= 64 pairs / 128 reads) while the CTA's groups fit one SM's shared memory
-   (one CTA of 2 or 3 groups per SM; with a single group, two CTAs per SM) */
+/* tile size: as large as possible (<= 128 pairs / 256 reads) while one CTA fits an SM's shared memory */
 static void make_smem_layout(fp_ctx* c) {
     const int sides = c->p.paired ? 2 : 1;
-    const size_t budget = (c->groups == 1 && c->group_threads == 256) ? (227 * 1024 - 2 * 1024) / 2 : (size_t)227 * 1024;
-    int T = 64 * (3 - sides) * (c->group_threads / 256);
-    if (T > (sides == 2 ? 128 : 256)) T = sides == 2 ? 128 : 256;   /* row indices: 7 bits in the correction list (PE), 8 bits in the removal lists */
+    const size_t budget = (size_t)227 * 1024;
+    int T = sides == 2 ? 128 : 256;                                 /* row indices: 7 bits in the correction list (PE), 8 bits in the removal lists */
     while (T > 16 && smem_layout_for_tile(c, T, c->sl) > budget) T -= 8;
     c->tile = T;
     smem_layout_for_tile(c, T, c->sl);
-    /* kernel variants that stay selectable for measurements (DESIGN.md section 5): bit 0 = base correction on per-warp work lists behind ONE
-       group barrier, bit 1 = L2 prefetch of the CTA's next tile (off: 1 - 1.5 % faster on every bench workload on an H100) */
-    c->sl.xflags = 0;
-    if (const char* e = getenv("FP_XFLAGS")) c->sl.xflags = atoi(e);
-    /* threads per column of the dense column pass (phase A's dense_tile, phase C's dense_remove): as many as fit in 5/8 of the group
+    /* threads per column of the dense column pass (phase A's dense_tile, phase C's dense_remove): as many as fit in 5/8 of the CTA
        (10 of 16 warps), at least one.  The column pass needs no item and no item needs it, so the warps without columns start the plane /
        histogram items at once and the column warps join them when their rows are done.  With every thread on columns (3 per column at
        2 x 150 bp, 2 at 2 x 250 bp) one warp or none started the items early; on an H100 10 column warps were best for PE and SE at stride
        160 and 8 for PE at stride 256 (DESIGN.md section 9) */
     const int ncols = sides * (c->stride / 2);
-    c->sl.col_split = std::max(1, c->group_threads * 5 / 8 / ncols);
+    c->sl.col_split = std::max(1, kChainThreads * 5 / 8 / ncols);
 }
 
 static int ctx_init(fp_ctx* c, const fp_params* p, int device, int64_t max_batch, int32_t stride, int32_t cycles);
@@ -312,9 +292,6 @@ static int ctx_init(fp_ctx* c, const fp_params* p, int device, int64_t max_batch
         CK(cudaFree(d_base));
         c->smem_base = h_base;
     }
-    if (const char* e = getenv("FP_GROUPS")) { const int g = atoi(e); if (g >= 1 && g <= 3) c->groups = g; }
-    if (const char* e = getenv("FP_GROUP_THREADS")) { if (atoi(e) == 256) { c->group_threads = 256; if (!getenv("FP_GROUPS")) c->groups = 2; } }
-    if (c->group_threads == 512) c->groups = 1;
     make_smem_layout(c);
 
     cudaDeviceProp prop;
@@ -437,13 +414,13 @@ static int ctx_init(fp_ctx* c, const fp_params* p, int device, int64_t max_batch
     /* kernel attributes + persistent grid size */
     int occ = 0;
     {
-        const void* fn = chain_kernel(p->paired != 0, c->groups, c->group_threads);
+        const void* fn = p->paired ? (const void*)fp_chain2_kernel<true> : (const void*)fp_chain2_kernel<false>;
         CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, c->sl.total));
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, c->group_threads * c->groups, c->sl.total));
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, kChainThreads, c->sl.total));
     }
     if (occ < 1) return set_err(FP_E_CUDA, "kernel cannot be resident (shared memory / registers)");
     c->grid_max = occ * c->num_sms;
-    if (getenv("FP_TRACE")) fprintf(stderr, "[fastp_b200] groups %d x %d threads, tile %d rows, smem %d B (shared %d + %d per group), %d CTA/SM, %d threads per column\n", c->groups, c->group_threads, c->tile, c->sl.total, c->sl.off_group, c->sl.group_stride, occ, c->sl.col_split);
+    if (getenv("FP_TRACE")) fprintf(stderr, "[fastp_b200] chain kernel: tile %d rows, smem %d B, %d CTA/SM, %d threads per column\n", c->tile, c->sl.total, occ, c->sl.col_split);
     return FP_OK;
 }
 
@@ -575,7 +552,7 @@ static int launch_chain(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
     a.counters = reinterpret_cast<unsigned long long*>(c->d_raw);
     a.n_tiles = (b->n + c->tile - 1) / c->tile;
     a.sl = c->sl;
-    int grid = (int)std::min<long long>((a.n_tiles + c->groups - 1) / c->groups, c->grid_max);
+    int grid = (int)std::min<long long>(a.n_tiles, c->grid_max);
     /* The operator parameters live in ONE __constant__ block per device, owned by the context that launched last.  A launch by the owner
        costs nothing; a launch by another context first waits -- on the device, in its own stream -- for the owner's last chain kernel
        (the only reader of the block), then rewrites the block from its device copy with a small kernel (stream-ordered, no copy engine:
@@ -619,7 +596,8 @@ static int launch_chain(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
     CK(cudaEventRecord(ev.a, st));
     {
         void* kargs[] = {(void*)&a};
-        CK(cudaLaunchKernel(chain_kernel(c->p.paired != 0, c->groups, c->group_threads), dim3(grid), dim3(c->group_threads * c->groups), kargs, (size_t)c->sl.total, st));
+        const void* fn = c->p.paired ? (const void*)fp_chain2_kernel<true> : (const void*)fp_chain2_kernel<false>;
+        CK(cudaLaunchKernel(fn, dim3(grid), dim3(kChainThreads), kargs, (size_t)c->sl.total, st));
     }
     CK(cudaEventRecord(ev.b, st));
     CK(cudaEventRecord(c->last_chain_ev, st));

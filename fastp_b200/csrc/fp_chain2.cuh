@@ -713,7 +713,7 @@ __device__ __noinline__ int t_correct(const TRead r1, const TRead r2, uint32_t* 
  * Base correction, distributed form (clean pairs).  A pair with a 3' low-quality tail inside its overlap can have dozens of
  * correctable positions; one lane working through them holds back its whole warp -- and, behind the tile's barrier, the CTA.
  * So the pair's lanes only DECIDE (which mismatching positions are rewritten, from the two quality bytes) and put every
- * correction on the tile's work list; then ONE LANE PER CORRECTION (all warps of the group) does the statistics deltas, the
+ * correction on the tile's work list; then ONE LANE PER CORRECTION (all warps of the CTA) does the statistics deltas, the
  * patch entry and, after a barrier, the rewrite.  Everything about one correction is independent of the others except the
  * 5-mer delta of corrections less than five bases apart on one read: each affected window (ending at x in [P, P+4]) is taken
  * by the LAST corrected position not beyond x (the per-row mask of corrected positions tells), with its old bases from the
@@ -1505,36 +1505,32 @@ __device__ __forceinline__ void push_delta(const DeltaSinks& K, bool want, bool 
 }
 
 /* ------------------------------------------------------------------------------------------------
- * The fused kernel, generation 2.  Per tile, separated by CTA barriers (phase-synchronous execution keeps the
- * instruction cache warm; two CTAs per SM overlap each other's barriers):
+ * The fused kernel, generation 2.  Persistent, one CTA of kChainThreads per SM, one tile at a time.  Per tile, separated by
+ * CTA barriers (phase-synchronous execution: every warp of the SM runs the same region of the kernel, which keeps the
+ * instruction cache warm):
  *   A  dense column pass (warps holding columns)  ||  bit planes + validation (the other warps)
  *   B  operator chain, one lane group per read / pair; post-stat requests go to a shared-memory queue
  *   C  the queue is drained by all warps (balanced), then the tile buffer is free for the next TMA load
  * ------------------------------------------------------------------------------------------------ */
-template <bool PAIRED, int NG, int CT>
-__global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_chain2_kernel(const fp_launch_args a) {
+static constexpr int kChainThreads = 512;         /* 16 warps: 128 registers each fill the SM's register file */
+template <bool PAIRED>
+__global__ void __launch_bounds__(kChainThreads, 1) fp_chain2_kernel(const fp_launch_args a) {
     extern __shared__ __align__(128) uint8_t smem[];
     constexpr int SIDES = PAIRED ? 2 : 1;
     const fp_smem_layout& sl = a.sl;
     const int S = c_p.stride, T = c_p.tile;
-    /* A CTA is NG independent tile pipelines ("groups") of CT threads each: own tile buffer, planes, queues, mbarrier and named
-       barrier; the histogram / delta / counter tables are shared by the groups (they are atomics anyway), which is what lets three
-       groups = 24 warps fit one SM's shared memory.  tid / warp are GROUP-local; ctid is the CTA-wide thread index. */
-    const int ctid = threadIdx.x, gid = NG == 1 ? 0 : (int)(threadIdx.x / CT);
-    const int tid = NG == 1 ? (int)threadIdx.x : (int)(threadIdx.x % CT), lane = lane_id(), warp = tid >> 5;
-    uint8_t* const gsm = smem + sl.off_group + gid * sl.group_stride;        /* this group's private region */
-#define GSYNC() asm volatile("bar.sync %0, %1;" :: "r"(1 + gid), "r"(CT) : "memory")
+    const int tid = threadIdx.x, lane = lane_id(), warp = tid >> 5;
     unsigned long long* G = a.counters;
     const fp_counter_layout& L = c_p.L;
 
-    uint64_t* mbar = reinterpret_cast<uint64_t*>(gsm + sl.off_mbar);
+    uint64_t* mbar = reinterpret_cast<uint64_t*>(smem + sl.off_mbar);
     uint8_t* tile_seq[2]; uint8_t* tile_qual[2];
-    tile_seq[0] = gsm + sl.off_tile;
+    tile_seq[0] = smem + sl.off_tile;
     tile_qual[0] = tile_seq[0] + sl.tile_array_bytes;
     tile_seq[1] = tile_qual[0] + sl.tile_array_bytes;
     tile_qual[1] = tile_seq[1] + sl.tile_array_bytes;
-    uint16_t* s_len = reinterpret_cast<uint16_t*>(gsm + sl.off_len);       /* [SIDES][T] */
-    uint8_t* s_clean = gsm + sl.off_clean;                                 /* [SIDES][T] */
+    uint16_t* s_len = reinterpret_cast<uint16_t*>(smem + sl.off_len);      /* [SIDES][T] */
+    uint8_t* s_clean = smem + sl.off_clean;                                /* [SIDES][T] */
     unsigned int* s_kmer = reinterpret_cast<unsigned int*>(smem + sl.off_kmer);    /* [SIDES][1024] */
     unsigned int* s_qhist = reinterpret_cast<unsigned int*>(smem + sl.off_qhist);  /* [SIDES][128][FP_QH_REP] */
     BlockCounters* bc = reinterpret_cast<BlockCounters*>(smem + sl.off_bc);
@@ -1543,7 +1539,7 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
     D.cyc = reinterpret_cast<int*>(smem + sl.off_delta);
     D.kmer = reinterpret_cast<int*>(smem + sl.off_dkmer);
     D.qh = reinterpret_cast<int*>(smem + sl.off_dqh);
-    uint32_t* s_rm = reinterpret_cast<uint32_t*>(gsm + sl.off_rm);          /* [SIDES][T + 4] removal lists */
+    uint32_t* s_rm = reinterpret_cast<uint32_t*>(smem + sl.off_rm);         /* [SIDES][T + 4] removal lists */
     int* s_nrm = reinterpret_cast<int*>(s_rm + SIDES * (T + 4));             /* [SIDES] their lengths */
     const int NBK = (S + 31) >> 5;                                           /* removal buckets per side: by lo >> 5 */
     uint32_t* s_bk = s_rm + SIDES * (T + 4) + 4;                             /* [SIDES][NBK][T + 4] */
@@ -1551,36 +1547,31 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
     DeltaSinks sinks; sinks.rm = s_rm; sinks.nrm = s_nrm; sinks.T = T;
     int16_t* s_lut = reinterpret_cast<int16_t*>(smem + sl.off_lut);
     const int PW = sl.plane_words, PSTR = sl.plane_stride;                  /* PSTR odd: conflict-free lane-group-per-row access */
-    uint32_t* tile_planes = reinterpret_cast<uint32_t*>(gsm + sl.off_planes);             /* [SIDES][T] rows of PSTR words */
-    DeltaReq* s_queue = reinterpret_cast<DeltaReq*>(gsm + sl.off_queue);    /* [SIDES * T * 2] */
+    uint32_t* tile_planes = reinterpret_cast<uint32_t*>(smem + sl.off_planes);            /* [SIDES][T] rows of PSTR words */
+    DeltaReq* s_queue = reinterpret_cast<DeltaReq*>(smem + sl.off_queue);   /* [SIDES * T * 2] */
     unsigned int* s_dummy = reinterpret_cast<unsigned int*>(smem + sl.off_dummy);   /* [32] write-only sink */
-    int* s_qn = reinterpret_cast<int*>(gsm + sl.off_next);                  /* [0] queue length, [1] pop cursor, [2] phase-A item cursor, [3] removal item cursor */
+    int* s_qn = reinterpret_cast<int*>(smem + sl.off_next);                 /* [0] queue length, [1] pop cursor, [2] phase-A item cursor, [3] removal item cursor */
     sinks.q = s_queue; sinks.qn = &s_qn[0];
-    uint32_t* s_corr = reinterpret_cast<uint32_t*>(gsm + sl.off_corr);      /* [FP_CORR_CAP] base-correction work list of the tile (PE) */
+    uint32_t* s_corr = reinterpret_cast<uint32_t*>(smem + sl.off_corr);     /* [FP_CORR_CAP] base-correction work list of the tile (PE) */
     int* s_ncorr = reinterpret_cast<int*>(s_corr + FP_CORR_CAP);            /* its length */
-    uint32_t* s_cm = reinterpret_cast<uint32_t*>(gsm + sl.off_cm);          /* [SIDES][T][CMW] corrected positions of every row */
+    uint32_t* s_cm = reinterpret_cast<uint32_t*>(smem + sl.off_cm);         /* [SIDES][T][CMW] corrected positions of every row */
     const int CMW = sl.cm_words;
 
     if (((smem_u32(smem) + (uint32_t)sl.off_kmer) & 4095u) != 0u) __trap();   /* layout was built for another shared-window base */
-    for (int i = tid; i < SIDES * T * PSTR; i += CT) tile_planes[i] = 0;
-    for (int i = ctid; i < SIDES * FP_KMER_BINS; i += CT * NG) s_kmer[i] = 0;
-    for (int i = ctid; i < SIDES * FP_QUAL_BINS * FP_QH_REP; i += CT * NG) s_qhist[i] = 0;
-    for (int i = ctid; i < SIDES * S * 20; i += CT * NG) D.cyc[i] = 0;
-    for (int i = ctid; i < SIDES * FP_KMER_BINS; i += CT * NG) D.kmer[i] = 0;
-    for (int i = ctid; i < SIDES * FP_QUAL_BINS; i += CT * NG) D.qh[i] = 0;
-    for (int i = ctid; i < (int)(sizeof(BlockCounters) / 4); i += CT * NG) reinterpret_cast<unsigned int*>(bc)[i] = 0;
-    for (int i = ctid; i < S + 2; i += CT * NG) { s_lut[i] = c_p.lut_ovlimit[i]; s_lut[(S + 2) + i] = c_p.lut_lowq[i]; s_lut[2 * (S + 2) + i] = c_p.lut_mindiff[i]; }
+    for (int i = tid; i < SIDES * T * PSTR; i += kChainThreads) tile_planes[i] = 0;
+    for (int i = tid; i < SIDES * FP_KMER_BINS; i += kChainThreads) s_kmer[i] = 0;
+    for (int i = tid; i < SIDES * FP_QUAL_BINS * FP_QH_REP; i += kChainThreads) s_qhist[i] = 0;
+    for (int i = tid; i < SIDES * S * 20; i += kChainThreads) D.cyc[i] = 0;
+    for (int i = tid; i < SIDES * FP_KMER_BINS; i += kChainThreads) D.kmer[i] = 0;
+    for (int i = tid; i < SIDES * FP_QUAL_BINS; i += kChainThreads) D.qh[i] = 0;
+    for (int i = tid; i < (int)(sizeof(BlockCounters) / 4); i += kChainThreads) reinterpret_cast<unsigned int*>(bc)[i] = 0;
+    for (int i = tid; i < S + 2; i += kChainThreads) { s_lut[i] = c_p.lut_ovlimit[i]; s_lut[(S + 2) + i] = c_p.lut_lowq[i]; s_lut[2 * (S + 2) + i] = c_p.lut_mindiff[i]; }
     if (tid == 0) { mbar_init(mbar, 1); s_qn[0] = 0; s_qn[1] = 0; s_qn[2] = 0; asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-    /* base correction work lists: ONE list per group (xflags bit 0 clear), or one per warp: region w = s_corr[w * WR .. (w+1) * WR), its
-       length in word 0 -- then nothing about a correction leaves the warp that decided it */
-    constexpr int WR = FP_CORR_CAP / (CT / 32);
-    const bool warp_lists = PAIRED && (sl.xflags & 1);
-    if (PAIRED) for (int i = tid; i < FP_CORR_CAP; i += CT) s_corr[i] = 0;
 
     /* column-pass ownership: thread = (side, half-word column): cycles 2*hc, 2*hc+1 */
     const int HPR = S >> 1;
-    const int ncols = SIDES * HPR;                /* host guarantees ncols <= CT */
-    const int nsplit = sl.col_split;              /* row groups are dealt round-robin to nsplit threads per column; host: 1 <= nsplit <= CT / ncols */
+    const int ncols = SIDES * HPR;                /* host guarantees ncols <= kChainThreads */
+    const int nsplit = sl.col_split;              /* row groups are dealt round-robin to nsplit threads per column; host: 1 <= nsplit <= kChainThreads / ncols */
     const bool col_active = tid < ncols * nsplit;
     const int my_part = tid / ncols, my_col = col_active ? tid % ncols : 0;     /* my_part is read by column threads only */
     const int my_side = my_col / HPR, my_hc = my_col % HPR;
@@ -1606,7 +1597,7 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
         if (t >= a.n_tiles) return;
         const long long r0 = t * T;
         const int nr = (int)min((long long)T, a.b.n - r0);
-        for (int i = tid; i < SIDES * T; i += CT) {
+        for (int i = tid; i < SIDES * T; i += kChainThreads) {
             const int sd = i / T, r = i % T;
             uint16_t ln = 0;
             if (r < nr) { ln = (sd == 0 ? a.b.len1 : a.b.len2)[r0 + r]; if (ln > S) ln = (uint16_t)S; }
@@ -1614,7 +1605,7 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
             s_clean[i] = 1;
         }
     };
-    fill_lens((long long)blockIdx.x * NG + gid);
+    fill_lens(blockIdx.x);
     __syncthreads();
     uint32_t parity = 0;
 #ifdef FP_PHASE_TIMING
@@ -1626,7 +1617,7 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
 #endif
 
     #pragma unroll 1
-    for (long long tix = (long long)blockIdx.x * NG + gid; tix < a.n_tiles; tix += (long long)gridDim.x * NG) {
+    for (long long tix = blockIdx.x; tix < a.n_tiles; tix += gridDim.x) {
         const long long row0 = tix * T;
         const int rows = (int)min((long long)T, a.b.n - row0);
         /* ---------------- TMA bulk loads ---------------- */
@@ -1641,13 +1632,6 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
                 tma_bulk_g2s(tile_qual[1], a.b.qual2 + row0 * S, bytes, mbar);
             }
             s_qn[0] = 0; s_qn[1] = 0; s_qn[3] = 0;     /* request queue / removal items: next used after the phase-A barrier */
-            const long long tnext = tix + (long long)gridDim.x * NG;               /* the tile this group loads next: into L2 while this one is worked on */
-            if ((sl.xflags & 2) && tnext < a.n_tiles) {
-                const long long rn0 = tnext * T;
-                const uint32_t nb = (uint32_t)min((long long)T, a.b.n - rn0) * (uint32_t)S;
-                l2_prefetch(a.b.seq1 + rn0 * S, nb); l2_prefetch(a.b.qual1 + rn0 * S, nb);
-                if (PAIRED) { l2_prefetch(a.b.seq2 + rn0 * S, nb); l2_prefetch(a.b.qual2 + rn0 * S, nb); }
-            }
             if (PAIRED && c_p.correction) *s_ncorr = 0;
         }
         /* the read lengths of this tile were staged before the previous tile's last barrier (fill_lens), the bytes arrive through the
@@ -1655,8 +1639,8 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
         mbar_wait(mbar, parity);
         FP_TP(0);
         parity ^= 1;
-        for (int i = tid; i < SIDES * (T + 4) + 4 + SIDES * NBK * (T + 4) + SIDES * NBK; i += CT) s_rm[i] = 0;      /* removal lists + lengths: filled in phase B */
-        if (PAIRED && c_p.correction) for (int i = tid; i < SIDES * T * CMW; i += CT) s_cm[i] = 0;
+        for (int i = tid; i < SIDES * (T + 4) + 4 + SIDES * NBK * (T + 4) + SIDES * NBK; i += kChainThreads) s_rm[i] = 0;      /* removal lists + lengths: filled in phase B */
+        if (PAIRED && c_p.correction) for (int i = tid; i < SIDES * T * CMW; i += kChainThreads) s_cm[i] = 0;
 
         /* ---------------- phase A: dense pass (column warps) || bit planes + validation (other warps) ---------------- */
         if (col_active)           /* dense column pass: pre-filter stats of every row of the tile, two cycles per thread */
@@ -1690,7 +1674,7 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
                     if (rr2 < rows) {
                         const int n = (int)s_len[sd * T + rr2] - 32 * j;
                         if (n > 0) {
-                            const uint8_t* tseq_sd = gsm + sl.off_tile + sd * 2 * sl.tile_array_bytes; const uint8_t* tqual_sd = tseq_sd + sl.tile_array_bytes;
+                            const uint8_t* tseq_sd = smem + sl.off_tile + sd * 2 * sl.tile_array_bytes; const uint8_t* tqual_sd = tseq_sd + sl.tile_array_bytes;
                             /* One pass over the chunk in four steps of 8 bases (two words): per-byte class flags of the even word in bit 0,
                                of the odd word in bit 4, so one multiply gathers 8 flags into the product's top byte (see plane_pair) and
                                PRMT shifts it into the plane word.  The same step packs the 2-bit base codes for the 5-mer windows and
@@ -1783,12 +1767,12 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
             }
         }
         FP_TP(1);
-        GSYNC();
+        __syncthreads();
         FP_TP(2);
 
         /* ---------------- phase B: operator chain, one lane GROUP per read / pair ---------------- */
         #pragma unroll 1
-        for (int rb0 = 0; rb0 < rows; rb0 += (CT / 32) * UPW) {            /* same trip count for every warp: the loop body holds group barriers */
+        for (int rb0 = 0; rb0 < rows; rb0 += (kChainThreads / 32) * UPW) { /* same trip count for every warp: the loop body holds CTA barriers */
             const int rbase = rb0 + warp * UPW;
             const int r = rbase + lane / GL;
             const bool active = r < rows;
@@ -1885,53 +1869,33 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
                     else ovA = ov;
                     need_correct = both && c_p.correction && !ovA.has_gap && ovA.overlapped && ovA.diff != 0;       /* :443,:453-456 */
                 }
-                /* ---- base correction (:453-456): the pairs' lanes decide, then the whole GROUP works the tile's list, one lane per correction.
-                        Group barriers on purpose: a per-warp variant (warp-level syncs only) is slower -- eight warps running the
-                        correction code at eight different times thrash the instruction cache, while
+                /* ---- base correction (:453-456): the pairs' lanes decide, then the whole CTA works the tile's list, one lane per correction.
+                        CTA barriers on purpose: a per-warp variant (warp-level syncs only) is slower -- warps running the
+                        correction code at different times thrash the instruction cache, while
                         phase-synchronous warps share one hot region at a time. ---- */
                 bool corr_overflow = false;
                 const bool distributed = need_correct && clean1 && clean2;
                 if (PAIRED && c_p.correction) {
-                    uint32_t* const wlist = warp_lists ? s_corr + warp * WR + 1 : s_corr;
-                    int* const wn = warp_lists ? reinterpret_cast<int*>(s_corr + warp * WR) : s_ncorr;
-                    const int wcap = warp_lists ? WR - 1 : FP_CORR_CAP;
                     if (distributed)
-                        corr_overflow = t_correct_decide(r1, r2, PW, ovA, rr, sub, GL, wlist, wn, wcap, s_cm + rr * CMW, s_cm + (T + rr) * CMW);
-                    /* the one barrier that stays: the warps leave the overlap analysis at very different times, and behind it they run the
+                        corr_overflow = t_correct_decide(r1, r2, PW, ovA, rr, sub, GL, s_corr, s_ncorr, FP_CORR_CAP, s_cm + rr * CMW, s_cm + (T + rr) * CMW);
+                    /* the warps leave the overlap analysis at very different times, and behind this barrier they run the
                        correction code TOGETHER (one hot region of the instruction cache) */
                     FP_TP(3);
-                    GSYNC();
+                    __syncthreads();
                     FP_TP(4);
-                    if (warp_lists) {
-                        /* a pair's rows, masks and planes belong to the warp that holds the pair: warp-level syncs order item -> apply -> chain */
-                        const int ncorr = min(*wn, wcap);
-                        for (int i = lane; i < ncorr; i += 32)
-                            t_correct_item(wlist[i], tile_seq[0], sl.tile_array_bytes, S, T, s_len, s_cm, CMW, D, bc, a.sink, (unsigned int)(row0 + (wlist[i] & 0x7F)));
-                        __syncwarp();
-                        for (int i = lane; i < ncorr; i += 32) {
-                            const uint32_t en = wlist[i];
-                            const int erow = en & 0x7F, ewhich = (en >> 7) & 1;
-                            t_correct_apply(en, tile_seq[0], sl.tile_array_bytes, S, T, tile_planes, PSTR, PW,
-                                            (ewhich ? a.b.seq2 : a.b.seq1) + (row0 + erow) * S, (ewhich ? a.b.qual2 : a.b.qual1) + (row0 + erow) * S);
-                        }
-                        __syncwarp();
-                        if (lane == 0) *wn = 0;
-                        __syncwarp();
-                    } else {
-                        const int ncorr = min(*s_ncorr, FP_CORR_CAP);
-                        for (int i = tid; i < ncorr; i += CT)
-                            t_correct_item(s_corr[i], tile_seq[0], sl.tile_array_bytes, S, T, s_len, s_cm, CMW, D, bc, a.sink, (unsigned int)(row0 + (s_corr[i] & 0x7F)));
-                        GSYNC();
-                        for (int i = tid; i < ncorr; i += CT) {
-                            const uint32_t en = s_corr[i];
-                            const int erow = en & 0x7F, ewhich = (en >> 7) & 1;
-                            t_correct_apply(en, tile_seq[0], sl.tile_array_bytes, S, T, tile_planes, PSTR, PW,
-                                            (ewhich ? a.b.seq2 : a.b.seq1) + (row0 + erow) * S, (ewhich ? a.b.qual2 : a.b.qual1) + (row0 + erow) * S);
-                        }
-                        GSYNC();
-                        FP_TP(5);
-                        if (tid == 0) *s_ncorr = 0;                /* (a PE tile is one round of this loop: 8 warps x 8 pairs >= T) */
+                    const int ncorr = min(*s_ncorr, FP_CORR_CAP);
+                    for (int i = tid; i < ncorr; i += kChainThreads)
+                        t_correct_item(s_corr[i], tile_seq[0], sl.tile_array_bytes, S, T, s_len, s_cm, CMW, D, bc, a.sink, (unsigned int)(row0 + (s_corr[i] & 0x7F)));
+                    __syncthreads();
+                    for (int i = tid; i < ncorr; i += kChainThreads) {
+                        const uint32_t en = s_corr[i];
+                        const int erow = en & 0x7F, ewhich = (en >> 7) & 1;
+                        t_correct_apply(en, tile_seq[0], sl.tile_array_bytes, S, T, tile_planes, PSTR, PW,
+                                        (ewhich ? a.b.seq2 : a.b.seq1) + (row0 + erow) * S, (ewhich ? a.b.qual2 : a.b.qual1) + (row0 + erow) * S);
                     }
+                    __syncthreads();
+                    FP_TP(5);
+                    if (tid == 0) *s_ncorr = 0;                    /* (a PE tile is one round of this loop: 16 warps x 8 pairs >= T) */
                 }
                 int res1 = FP_FAIL_LENGTH, res2 = FP_FAIL_LENGTH;
                 bool counted = false;
@@ -2077,7 +2041,7 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
         }
 
         FP_TP(6);
-        GSYNC();
+        __syncthreads();
         FP_TP(7);
 
         /* ---------------- phase C: post-filter statistics of what the chain removed / shifted (all warps) ---------------- */
@@ -2111,7 +2075,7 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
                         const int row = e & 0xFF, lo = (e >> 8) & 0xFFF, hi = e >> 20;
                         const int a0 = max(lo - 32 * j, 0), b0 = min(hi - 32 * j, 32);
                         if (b0 > a0) {
-                            const uint8_t* sp = gsm + sl.off_tile + sd * 2 * sl.tile_array_bytes + row * S + 32 * j;
+                            const uint8_t* sp = smem + sl.off_tile + sd * 2 * sl.tile_array_bytes + row * S + 32 * j;
                             const uint32_t* pnn = tile_planes + (sd * T + row) * PSTR + 2 * PW;
                             hist_remove_chunk(sp, sp + sl.tile_array_bytes, j, low_mask(b0) & ~low_mask(a0), pnn[j], j > 0 ? pnn[j - 1] : 0u,
                                               smem_u32(D.qh) + (uint32_t)sd * (FP_QUAL_BINS * 4), smem_u32(D.kmer) + (uint32_t)sd * (FP_KMER_BINS * 4), kdummy);
@@ -2131,15 +2095,15 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
                 const DeltaReq rq = s_queue[qi];
                 const int row = rq.a & 0xFF, side = (rq.a >> 8) & 1, sign = ((rq.a >> 10) & 1) ? -1 : +1;
                 const int ctx0 = (int)(rq.a >> 12), rlo = (int)(rq.b & 0xFFFF), rhi = (int)(rq.b >> 16);
-                const uint8_t* sq = gsm + sl.off_tile + side * 2 * sl.tile_array_bytes + row * S; const uint8_t* ql = sq + sl.tile_array_bytes;
+                const uint8_t* sq = smem + sl.off_tile + side * 2 * sl.tile_array_bytes + row * S; const uint8_t* ql = sq + sl.tile_array_bytes;
                 if ((rq.a >> 9) & 1) dev_stat_positions_smem(D, side, sq, ql, ctx0, rlo, rhi, sign);
                 else dev_stat_positions(G, side * 2 + 1, sq, ql, ctx0, rlo, rhi, sign);
             }
         }
-        fill_lens(tix + (long long)gridDim.x * NG);
+        fill_lens(tix + gridDim.x);
         if (tid == 0) s_qn[2] = 0;                     /* item counter of phase A: idle since the phase-A barrier */
         FP_TP(8);
-        GSYNC();
+        __syncthreads();
         FP_TP(9);
     }
 
@@ -2148,7 +2112,7 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
         printf("PHASE warp %2d col %d tma %lld colA %lld itemsA %lld totA %lld busyB1 %lld totB1 %lld corr %lld busyB2 %lld totB2 %lld colC %lld itemsC %lld totC %lld\n",
                warp, col_active ? 1 : 0, tph[0], tph[10], tph[1], tph[2], tph[3], tph[4], tph[5], tph[6], tph[7], tph[11], tph[8], tph[9]);
 #endif
-    __syncthreads();                               /* every group is done with the shared tables */
+    __syncthreads();                               /* every warp is done with the shared tables */
     /* ---------------- flush block-level accumulators ---------------- */
     const int BIN_SLOT[NB] = {1, 3, 4, 6, 7};      /* base & 7 of A C T N G */
     if (col_active) {
@@ -2173,19 +2137,19 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
         }
     }
     #pragma unroll 1
-    for (int i = ctid; i < SIDES * FP_KMER_BINS; i += CT * NG) {
+    for (int i = tid; i < SIDES * FP_KMER_BINS; i += kChainThreads) {
         const unsigned int v = s_kmer[i];
         if (v) { const int sd = i / FP_KMER_BINS, k = kmer_ref_index(i % FP_KMER_BINS); red_add64(&G[fp_off_kmer(&L, sd * 2, k)], (unsigned long long)v); red_add64(&G[fp_off_kmer(&L, sd * 2 + 1, k)], (unsigned long long)v); }
     }
     #pragma unroll 1
-    for (int i = ctid; i < SIDES * FP_QUAL_BINS; i += CT * NG) {
+    for (int i = tid; i < SIDES * FP_QUAL_BINS; i += kChainThreads) {
         unsigned int v = 0;
         #pragma unroll
         for (int c = 0; c < FP_QH_REP; c++) v += s_qhist[i * FP_QH_REP + c];
         if (v) { const int sd = i / FP_QUAL_BINS, k = i % FP_QUAL_BINS; red_add64(&G[fp_off_qualhist(&L, sd * 2, k)], (unsigned long long)v); red_add64(&G[fp_off_qualhist(&L, sd * 2 + 1, k)], (unsigned long long)v); }
     }
     #pragma unroll 1
-    for (int i = ctid; i < SIDES * S * 20; i += CT * NG) {
+    for (int i = tid; i < SIDES * S * 20; i += kChainThreads) {
         const int v = D.cyc[i];
         if (v == 0) continue;
         const int sd = i / (S * 20), rem = i % (S * 20), cyc = rem / 20, bin = (rem % 20) / 4, kind = rem & 3;
@@ -2194,17 +2158,17 @@ __global__ void __launch_bounds__(CT * NG, (NG == 1 && CT == 256) ? 2 : 1) fp_ch
         red_add64(&G[fp_off_cycle(&L, sd * 2 + 1, gk * 8 + BIN_SLOT[bin], cyc)], (unsigned long long)(long long)v);
     }
     #pragma unroll 1
-    for (int i = ctid; i < SIDES * FP_KMER_BINS; i += CT * NG) { const int v = D.kmer[i]; if (v) red_add64(&G[fp_off_kmer(&L, (i / FP_KMER_BINS) * 2 + 1, kmer_ref_index(i % FP_KMER_BINS))], (unsigned long long)(long long)v); }
+    for (int i = tid; i < SIDES * FP_KMER_BINS; i += kChainThreads) { const int v = D.kmer[i]; if (v) red_add64(&G[fp_off_kmer(&L, (i / FP_KMER_BINS) * 2 + 1, kmer_ref_index(i % FP_KMER_BINS))], (unsigned long long)(long long)v); }
     #pragma unroll 1
-    for (int i = ctid; i < SIDES * FP_QUAL_BINS; i += CT * NG) { const int v = D.qh[i]; if (v) red_add64(&G[fp_off_qualhist(&L, (i / FP_QUAL_BINS) * 2 + 1, i % FP_QUAL_BINS)], (unsigned long long)(long long)v); }
+    for (int i = tid; i < SIDES * FP_QUAL_BINS; i += kChainThreads) { const int v = D.qh[i]; if (v) red_add64(&G[fp_off_qualhist(&L, (i / FP_QUAL_BINS) * 2 + 1, i % FP_QUAL_BINS)], (unsigned long long)(long long)v); }
     #pragma unroll 1
-    for (int i = ctid; i < FP_FR_WORDS; i += CT * NG) { const unsigned int v = bc->fr[i]; if (v) red_add64(&G[L.off_filter + i], (unsigned long long)v); }
+    for (int i = tid; i < FP_FR_WORDS; i += kChainThreads) { const unsigned int v = bc->fr[i]; if (v) red_add64(&G[L.off_filter + i], (unsigned long long)v); }
     if (c_p.isize_max < FP_MAX_ISIZE_SMEM) {
         #pragma unroll 1
-        for (int i = ctid; i <= c_p.isize_max; i += CT * NG) { const unsigned int v = bc->isize[i]; if (v) red_add64(&G[L.off_isize + i], (unsigned long long)v); }
+        for (int i = tid; i <= c_p.isize_max; i += kChainThreads) { const unsigned int v = bc->isize[i]; if (v) red_add64(&G[L.off_isize + i], (unsigned long long)v); }
     }
-    if (ctid < 2 * L.n_stats && ctid < 8) {
-        const unsigned long long v = bc->rl[ctid];
-        if (v) red_add64(&G[(ctid & 1) ? fp_off_length_sum(&L, ctid >> 1) : fp_off_reads(&L, ctid >> 1)], v);
+    if (tid < 2 * L.n_stats && tid < 8) {
+        const unsigned long long v = bc->rl[tid];
+        if (v) red_add64(&G[(tid & 1) ? fp_off_length_sum(&L, tid >> 1) : fp_off_reads(&L, tid >> 1)], v);
     }
 }

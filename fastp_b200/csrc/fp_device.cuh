@@ -16,8 +16,6 @@
 
 #define FP_THREADS 256
 #define FP_WARPS (FP_THREADS / 32)
-#define FP_CT 256              /* threads of the chain kernel: 2 CTAs x 8 warps per SM (128 registers); 320 x 96 registers was measured and lost to spills */
-#define FP_CW (FP_CT / 32)
 #define FULL_MASK 0xffffffffu
 #define FP_MAX_ISIZE_SMEM 1025
 
@@ -375,8 +373,8 @@ __device__ __noinline__ void dev_stat_positions_smem(const DeltaAcc D, int side,
 struct fp_smem_layout {
     int off_dummy, off_mbar, off_next, off_tile, tile_array_bytes, off_len, off_clean, off_kmer, off_qhist, off_bc, off_lut, off_delta,
         off_dkmer, off_dqh, off_rm, off_planes, off_queue, plane_words, plane_stride, total,
-        off_group, group_stride, off_corr, off_cm, cm_words, xflags,     /* off_mbar, off_next, off_len, off_clean, off_tile, off_rm, off_planes, off_queue are relative to a group's region */
-        col_split;                   /* threads per column of the dense column pass, 1 .. CT / (sides * stride / 2) (fp_api.cu make_smem_layout) */
+        off_corr, off_cm, cm_words,
+        col_split;                   /* threads per column of the dense column pass, 1 .. kChainThreads / (sides * stride / 2) (fp_api.cu make_smem_layout) */
 };
 
 struct fp_launch_args {
@@ -406,10 +404,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     } while (!ok);
 }
 /* TMA bulk copy global -> shared (1-D), completion signalled on the mbarrier */
-/* bulk prefetch of a global span into L2 (bytes: a multiple of 16) */
-__device__ __forceinline__ void l2_prefetch(const void* src, uint32_t bytes) {
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" :: "l"(src), "r"(bytes) : "memory");
-}
 __device__ __forceinline__ void tma_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");

@@ -2,7 +2,7 @@
 # phase timing on an H100: swaps in the -DFP_PHASE_TIMING build (scripts/timing/libfastp_b200.so), prints what the 16 warps of CTA 0
 # spent per phase, then their means in M cycles.  Phases A and C are split into the dense column pass ("col": mean over the warps that
 # hold columns, measured up to the end of dense_tile / dense_remove), the items that follow it ("items": mean over all warps) and the
-# wait at the group barrier ("wait").  The bench logs go to $OUT (default: a new temporary directory).
+# wait at the CTA barrier ("wait").  The bench logs go to $OUT (default: a new temporary directory).
 OUT="${OUT:-$(mktemp -d)}"; mkdir -p "$OUT"
 [ -f scripts/timing/libfastp_b200.so ] || { echo "build it first: nvcc ... -DFP_PHASE_TIMING ... -o scripts/timing/libfastp_b200.so (same line as __graft_entry__.build)"; exit 1; }
 cp fastp_b200/libfastp_b200.so /tmp/lib_orig.so; cp scripts/timing/libfastp_b200.so fastp_b200/libfastp_b200.so

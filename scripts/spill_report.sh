@@ -1,8 +1,8 @@
 #!/bin/bash
 # Register spills of the hot kernel, on the CPU (no GPU needed): compiles fastp_b200/csrc/fp_api.cu to a cubin with the flags of
 # __graft_entry__.build() and prints
-#   * the ptxas stack / spill figures of every fp_chain2_kernel instantiation and of its out-of-line callees,
-#   * the local-memory loads / stores (LDL / STL) per source line of the default PE and SE kernels <PAIRED, 1, 512> with their callees;
+#   * the ptxas stack / spill figures of the PE and SE fp_chain2_kernel<PAIRED> and of their out-of-line callees,
+#   * the local-memory loads / stores (LDL / STL) per source line of both kernels with their callees;
 #     "loop" counts the ones inside a loop of the machine code (between a backward branch and its target).
 # Usage: scripts/spill_report.sh [arch, default sm_90a] [nvcc flags ...]     e.g.  scripts/spill_report.sh sm_100a
 set -euo pipefail
@@ -61,7 +61,7 @@ for ln in open(sass):
     if m: funcs[cur]["labels"][m.group(1)] = len(funcs[cur]["ins"]); continue
     m = re.match(r"\s*/\*([0-9a-f]+)\*/\s+(.*?);", ln)
     if m: funcs[cur]["ins"].append((line_of, m.group(2)))
-for want in ("_Z16fp_chain2_kernelILb1ELi1ELi512EEv14fp_launch_args", "_Z16fp_chain2_kernelILb0ELi1ELi512EEv14fp_launch_args"):
+for want in ("_Z16fp_chain2_kernelILb1EEv14fp_launch_args", "_Z16fp_chain2_kernelILb0EEv14fp_launch_args"):
     mine = [f for f in funcs if f == want or f.startswith("$" + want + "$")]
     per, tot = collections.Counter(), collections.Counter()
     for f in mine:

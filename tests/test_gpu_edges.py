@@ -123,7 +123,7 @@ def run_pe_device(gpu, ctx, t, n, patch_cap):
 
 @pytest.mark.parametrize("limit", [5, 20])
 def test_correction_overflow_device(gpu, limit):
-    """More corrections than a tile's work list holds (FP_CORR_CAP = 1024 per 128 pairs; 63 per warp): the rest of a pair is
+    """More corrections than a tile's work list holds (FP_CORR_CAP = 1024 per 128 pairs): the rest of a pair is
     corrected by the sequential path after part of it went through the list.  Then a patch list of 16 entries: the rows and
     counters are the same and the count still covers every correction.  fp_patches_undo restores the pristine rows."""
     n = 4000
