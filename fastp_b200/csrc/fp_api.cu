@@ -866,6 +866,8 @@ static int ensure_staging(fp_ctx* c) {
 static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_read_result* out2, fp_ov_result* ov,
                         fp_patch* hp_out = nullptr, uint64_t hp_cap = 0, uint64_t* hp_n = nullptr, const fp_packed_batch* pk = nullptr) {
     if (hp_n) *hp_n = 0;
+    /* the chain indexes the flags by the unit's index in its LAUNCH, and a host batch is launched chunk by chunk */
+    if (c->dup_flags) return set_err(FP_E_INVAL, "duplicate flags are set (fp_set_dup_flags): they belong to one fp_process_se / _pe launch, not to a host batch");
     CK(cudaSetDevice(c->device));
     int rc = ensure_staging(c);
     if (rc) return rc;
@@ -1397,6 +1399,7 @@ extern "C" int fp_fastq_process_host(fp_ctx* c, const uint8_t* text1, int64_t nb
     if (!c || !n_units || !consumed1 || !out_bytes1) return set_err(FP_E_INVAL, "null argument");
     const int sides = c->p.paired ? 2 : 1;
     if (sides == 2 && (!consumed2 || !out_bytes2)) return set_err(FP_E_INVAL, "paired ctx needs the second side");
+    if (c->dup_flags) return set_err(FP_E_INVAL, "duplicate flags are set (fp_set_dup_flags): the text path runs its own duplicate filter (fp_fastq_set_dedup)");
     CK(cudaSetDevice(c->device));
     cudaStream_t st = c->stream[0], up = c->stream[1];
     if (!c->fq_stream_out) {

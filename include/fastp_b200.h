@@ -467,7 +467,12 @@ int  fp_dup_totals(fp_ctx* ctx, int64_t* total, int64_t* dups);
 int  fp_dup_reset(fp_ctx* ctx);
 /* --dedup (src/options.h duplicate.dedup): `d_is_dup` = DEVICE flags of the batch the next fp_process_se / _pe call works on (as fp_dup_check
  * wrote them); flagged units keep their verdict counters but are left out of the post-filter stats and marked FP_F_DUPLICATE, which
- * fp_fastq_encode skips.  NULL switches it off.  fp_fastq_set_dedup: the text path (fp_fastq_process_host) runs the duplicate filter at
+ * fp_fastq_encode skips.  NULL switches it off.  The pointer stays set until it is changed: d_is_dup[i] belongs to unit i of the LAUNCH, so
+ * a caller that splits a stream over several launches sets it before each one to that launch's first unit, and clears it when done.
+ * In merging mode a merged read is counted and written whatever its flag says (src/peprocessor.cpp:528-534); only pairs that did not
+ * merge consult it (:547, :553, :575).  The host entry points (fp_process_*_host, _host_packed, _host_patches, fp_fastq_process_host)
+ * split their input into chunks and rounds of their own, so one flag array cannot follow them: while a pointer is set they return
+ * FP_E_INVAL and touch nothing.  fp_fastq_set_dedup: the text path (fp_fastq_process_host) runs the duplicate filter at
  * `accuracy_level` on every round's decoded rows before the chain (0 = off) and drops duplicates from the output when `dedup` is set. */
 int  fp_set_dup_flags(fp_ctx* ctx, const uint8_t* d_is_dup);
 int  fp_fastq_set_dedup(fp_ctx* ctx, int32_t accuracy_level, int32_t dedup);

@@ -576,11 +576,11 @@ static void fill_result(fp_read_result* o, const oread* r, const uint8_t* row, i
  * SingleEndProcessor::processSingleEnd loop body  src/seprocessor.cpp:204-296
  * ------------------------------------------------------------------------------------------ */
 static void process_se_one(const fp_params* p, const fp_counter_layout* L, int64_t* C,
-                           uint8_t* seq, uint8_t* qual, int len, fp_read_result* out) {
+                           uint8_t* seq, uint8_t* qual, int len, int dedupOut, fp_read_result* out) {
     int64_t* FR = C + L->off_filter;
     stat_read(p, C, L, FP_STATS_PRE1, seq, qual, len);                     /* :211 */
     oread r = {seq, qual, len, 0};
-    int frontTrimmed = 0, flags = 0, apos = 0, abases = 0, polyBase = 255, polyLen = 0;
+    int frontTrimmed = 0, flags = dedupOut ? FP_F_DUPLICATE : 0, apos = 0, abases = 0, polyBase = 255, polyLen = 0;
     if (!trim_and_cut(p, &r, p->trim_front1, p->trim_tail1, &frontTrimmed)) r.is_null = 1;   /* :235 */
     if (!r.is_null && p->polyg_enabled)                                 /* :237-240 */
         if (trim_polyg(&r, p->polyg_min_len)) flags |= FP_F_POLYG_TRIMMED;
@@ -605,17 +605,17 @@ static void process_se_one(const fp_params* p, const fp_counter_layout* L, int64
     int result = pass_filter(p, &r);                                    /* :273 */
     if (isAdapterDimer) { result = FP_FAIL_ADAPTER_DIMER; flags |= FP_F_ADAPTER_DIMER; }   /* :275-276 */
     FR[FP_FR_READSTATS + result] += 1;                                  /* :278 */
-    if (!r.is_null && result == FP_PASS_FILTER)                         /* :281-286 */
+    if (!dedupOut && !r.is_null && result == FP_PASS_FILTER)            /* :280-286 */
         stat_read(p, C, L, FP_STATS_POST1, r.seq, r.qual, r.len);
     fill_result(out, &r, seq, result, result, flags, apos, abases, polyBase, polyLen);
 }
 
 /* ------------------------------------------------------------------------------------------
- * PairEndProcessor::processPairEnd loop body  src/peprocessor.cpp:383-643 (incl. merging mode :519-560; no overlapped_out /
- * dedup / index filter / UMI) + statInsertSize :710-723
+ * PairEndProcessor::processPairEnd loop body  src/peprocessor.cpp:383-643 (incl. merging mode :519-560 and dedupOut :397-401;
+ * no overlapped_out / index filter / UMI) + statInsertSize :710-723
  * ------------------------------------------------------------------------------------------ */
 static void process_pe_one(const fp_params* p, const fp_counter_layout* L, int64_t* C,
-                           uint8_t* seq1, uint8_t* qual1, int len1, uint8_t* seq2, uint8_t* qual2, int len2,
+                           uint8_t* seq1, uint8_t* qual1, int len1, uint8_t* seq2, uint8_t* qual2, int len2, int dedupOut,
                            fp_read_result* out1, fp_read_result* out2, fp_ov_result* ovOut) {
     int64_t* FR = C + L->off_filter;
     int64_t* ISZ = C + L->off_isize;
@@ -623,7 +623,7 @@ static void process_pe_one(const fp_params* p, const fp_counter_layout* L, int64
     stat_read(p, C, L, FP_STATS_PRE2, seq2, qual2, len2);
     oread r1 = {seq1, qual1, len1, 0}, r2 = {seq2, qual2, len2, 0};
     int ft1 = 0, ft2 = 0;
-    int flags1 = 0, flags2 = 0, apos1 = 0, apos2 = 0, ab1 = 0, ab2 = 0, pb1 = 255, pb2 = 255, pl1 = 0, pl2 = 0;
+    int flags1 = dedupOut ? FP_F_DUPLICATE : 0, flags2 = flags1, apos1 = 0, apos2 = 0, ab1 = 0, ab2 = 0, pb1 = 255, pb2 = 255, pl1 = 0, pl2 = 0;
     if (!trim_and_cut(p, &r1, p->trim_front1, p->trim_tail1, &ft1)) r1.is_null = 1;   /* :425-426 */
     if (!trim_and_cut(p, &r2, p->trim_front2, p->trim_tail2, &ft2)) r2.is_null = 1;
     int both = !r1.is_null && !r2.is_null;
@@ -733,7 +733,7 @@ static void process_pe_one(const fp_params* p, const fp_counter_layout* L, int64
             oread m = {mseq, mqual, mlen1 + mlen2, 0};
             const int result = pass_filter(p, &m);                      /* :526 */
             FR[FP_FR_READSTATS + result] += 2;                          /* :527 */
-            if (result == FP_PASS_FILTER) {                             /* :528-534 */
+            if (result == FP_PASS_FILTER) {                             /* :528-534: dedupOut is not consulted for a merged read */
                 stat_read(p, C, L, FP_STATS_POST1, mseq, mqual, m.len);
                 FR[FP_FR_MERGED_PAIRS] += 1;                            /* mergedCount -> addMergedPairs :694 */
             }
@@ -748,9 +748,9 @@ static void process_pe_one(const fp_params* p, const fp_counter_layout* L, int64
                 flags1 |= FP_F_ADAPTER_DIMER; flags2 |= FP_F_ADAPTER_DIMER;
             }
             FR[FP_FR_READSTATS + result1] += 1;
-            if (result1 == FP_PASS_FILTER) stat_read(p, C, L, FP_STATS_POST1, r1.seq, r1.qual, r1.len);
+            if (result1 == FP_PASS_FILTER && !dedupOut) stat_read(p, C, L, FP_STATS_POST1, r1.seq, r1.qual, r1.len);   /* :547 */
             FR[FP_FR_READSTATS + result2] += 1;
-            if (result2 == FP_PASS_FILTER) stat_read(p, C, L, FP_STATS_POST1, r2.seq, r2.qual, r2.len);   /* read 2 into read 1's Stats: :555 */
+            if (result2 == FP_PASS_FILTER && !dedupOut) stat_read(p, C, L, FP_STATS_POST1, r2.seq, r2.qual, r2.len);   /* :553; read 2 into read 1's Stats: :555 */
             pv = imax(result1, result2);
             mergeProcessed = 1;
         }
@@ -764,7 +764,7 @@ static void process_pe_one(const fp_params* p, const fp_counter_layout* L, int64
         }
         pv = imax(result1, result2);
         FR[FP_FR_READSTATS + pv] += 2;                                  /* :573 */
-        if (!p->merge_enabled && !r1.is_null && result1 == FP_PASS_FILTER && !r2.is_null && result2 == FP_PASS_FILTER) {   /* :577-591 */
+        if (!dedupOut && !p->merge_enabled && !r1.is_null && result1 == FP_PASS_FILTER && !r2.is_null && result2 == FP_PASS_FILTER) {   /* :575-591 */
             stat_read(p, C, L, FP_STATS_POST1, r1.seq, r1.qual, r1.len);
             stat_read(p, C, L, FP_STATS_POST2, r2.seq, r2.qual, r2.len);
         }
@@ -775,8 +775,8 @@ static void process_pe_one(const fp_params* p, const fp_counter_layout* L, int64
     (void)ovComputed;
 }
 
-int fp_oracle_process(const fp_params* p, const fp_counter_layout* L, const fp_batch* b,
-                      fp_read_result* out1, fp_read_result* out2, fp_ov_result* ov, int64_t* counters) {
+int fp_oracle_process_dedup(const fp_params* p, const fp_counter_layout* L, const fp_batch* b, const uint8_t* is_dup,
+                            fp_read_result* out1, fp_read_result* out2, fp_ov_result* ov, int64_t* counters) {
     if (!p || !L || !b || !out1 || !counters) return FP_E_INVAL;
     if (b->stride > FP_MAX_STRIDE) return FP_E_INVAL;
     if (p->paired) {
@@ -784,13 +784,18 @@ int fp_oracle_process(const fp_params* p, const fp_counter_layout* L, const fp_b
         for (int64_t i = 0; i < b->n; i++)
             process_pe_one(p, L, counters,
                            b->seq1 + i * b->stride, b->qual1 + i * b->stride, b->len1[i],
-                           b->seq2 + i * b->stride, b->qual2 + i * b->stride, b->len2[i],
+                           b->seq2 + i * b->stride, b->qual2 + i * b->stride, b->len2[i], is_dup && is_dup[i],
                            out1 + i, out2 + i, ov ? ov + i : NULL);
     } else {
         for (int64_t i = 0; i < b->n; i++)
-            process_se_one(p, L, counters, b->seq1 + i * b->stride, b->qual1 + i * b->stride, b->len1[i], out1 + i);
+            process_se_one(p, L, counters, b->seq1 + i * b->stride, b->qual1 + i * b->stride, b->len1[i], is_dup && is_dup[i], out1 + i);
     }
     return FP_OK;
+}
+
+int fp_oracle_process(const fp_params* p, const fp_counter_layout* L, const fp_batch* b,
+                      fp_read_result* out1, fp_read_result* out2, fp_ov_result* ov, int64_t* counters) {
+    return fp_oracle_process_dedup(p, L, b, NULL, out1, out2, ov, counters);
 }
 
 /* Single-function entry points for known-answer tests (tests/test_oracle_kat.py). */
@@ -886,12 +891,13 @@ int fp_oracle_fastq_decode(const uint8_t* text, int64_t nbytes, int final_chunk,
     return 0;
 }
 
-/* Read::appendToString  src/read.cpp:119-134 for every read whose pair verdict is PASS (peprocessor.cpp:583-584) */
+/* Read::appendToString  src/read.cpp:119-134 for every read whose pair verdict is PASS and that --dedup did not flag
+ * (peprocessor.cpp:575-584, seprocessor.cpp:280-282) */
 int64_t fp_oracle_fastq_encode(const uint8_t* text, const fp_fastq_rec* recs, const fp_read_result* res, const uint8_t* seq, const uint8_t* qual,
                                int stride, int64_t n, uint8_t* out, int64_t out_cap) {
     int64_t o = 0;
     for (int64_t i = 0; i < n; i++) {
-        if (res[i].pair_verdict != FP_PASS_FILTER) continue;
+        if (res[i].pair_verdict != FP_PASS_FILTER || (res[i].flags & FP_F_DUPLICATE)) continue;
         const int64_t need = (int64_t)recs[i].name_len + recs[i].strand_len + 2 * (int64_t)res[i].len + 4;
         if (o + need <= out_cap) {
             uint8_t* d = out + o;

@@ -132,11 +132,11 @@ void copy_back(Read* r, int front, uint8_t* seq, uint8_t* qual) {
     memcpy(qual + front, r->mQuality->data(), r->length());
 }
 
-void se_one(Worker& w, const fp_params* p, uint8_t* seq, uint8_t* qual, int len, fp_read_result* out) {
+void se_one(Worker& w, const fp_params* p, uint8_t* seq, uint8_t* qual, int len, bool dedupOut, fp_read_result* out) {
     Options* mOptions = &w.opt;
     Read* or1 = make_read(seq, qual, len);
     w.pre1->statRead(or1);                                                    // seprocessor.cpp:211
-    int frontTrimmed = 0, flags = 0, polyBase = 255, polyLen = 0;
+    int frontTrimmed = 0, flags = dedupOut ? FP_F_DUPLICATE : 0, polyBase = 255, polyLen = 0;
     Read* r1 = w.filter->trimAndCut(or1, mOptions->trim.front1, mOptions->trim.tail1, frontTrimmed);   // :235
     if (r1 != NULL && mOptions->polyGTrim.enabled) {                          // :237-240
         int before = r1->length();
@@ -164,13 +164,13 @@ void se_one(Worker& w, const fp_params* p, uint8_t* seq, uint8_t* qual, int len,
     int result = w.filter->passFilter(r1);                                    // :273
     if (isAdapterDimer) { result = FAIL_ADAPTER_DIMER; flags |= FP_F_ADAPTER_DIMER; }
     w.fr->addFilterResult(result, 1);                                         // :278
-    if (r1 != NULL && result == PASS_FILTER) w.post1->statRead(r1);           // :281-286
+    if (!dedupOut && r1 != NULL && result == PASS_FILTER) w.post1->statRead(r1);   // :280-286
     fill_result(out, r1, len, frontTrimmed, result, result, flags, abases, polyBase, polyLen);
     (void)p;
     delete or1;   // r1 == or1 or NULL (trimAndCut mutates in place)
 }
 
-void pe_one(Worker& w, const fp_params* p, uint8_t* seq1, uint8_t* qual1, int len1, uint8_t* seq2, uint8_t* qual2, int len2,
+void pe_one(Worker& w, const fp_params* p, uint8_t* seq1, uint8_t* qual1, int len1, uint8_t* seq2, uint8_t* qual2, int len2, bool dedupOut,
             fp_read_result* out1, fp_read_result* out2, fp_ov_result* ovOut) {
     Options* mOptions = &w.opt;
     const bool tid0 = p->thread0_semantics != 0;
@@ -179,7 +179,7 @@ void pe_one(Worker& w, const fp_params* p, uint8_t* seq1, uint8_t* qual1, int le
     w.pre1->statRead(or1);                                                    // peprocessor.cpp:393-394
     w.pre2->statRead(or2);
     int frontTrimmed1 = 0, frontTrimmed2 = 0;
-    int flags1 = 0, flags2 = 0, pb1 = 255, pb2 = 255, pl1 = 0, pl2 = 0, ab1 = 0, ab2 = 0;
+    int flags1 = dedupOut ? FP_F_DUPLICATE : 0, flags2 = flags1, pb1 = 255, pb2 = 255, pl1 = 0, pl2 = 0, ab1 = 0, ab2 = 0;   // :397-401
     Read* r1 = w.filter->trimAndCut(or1, mOptions->trim.front1, mOptions->trim.tail1, frontTrimmed1);   // :425-426
     Read* r2 = w.filter->trimAndCut(or2, mOptions->trim.front2, mOptions->trim.tail2, frontTrimmed2);
     if (r1 != NULL && r2 != NULL && mOptions->polyGTrim.enabled) {            // :428-431
@@ -280,9 +280,9 @@ void pe_one(Worker& w, const fp_params* p, uint8_t* seq1, uint8_t* qual1, int le
             result2 = w.filter->passFilter(r2);
             if (isAdapterDimer) { result1 = FAIL_ADAPTER_DIMER; result2 = FAIL_ADAPTER_DIMER; flags1 |= FP_F_ADAPTER_DIMER; flags2 |= FP_F_ADAPTER_DIMER; }
             w.fr->addFilterResult(result1, 1);
-            if (result1 == PASS_FILTER) w.post1->statRead(r1);
+            if (result1 == PASS_FILTER && !dedupOut) w.post1->statRead(r1);   // :547
             w.fr->addFilterResult(result2, 1);
-            if (result2 == PASS_FILTER) w.post1->statRead(r2);
+            if (result2 == PASS_FILTER && !dedupOut) w.post1->statRead(r2);   // :553
             pv = std::max(result1, result2);
             mergeProcessed = true;
         }
@@ -293,7 +293,7 @@ void pe_one(Worker& w, const fp_params* p, uint8_t* seq1, uint8_t* qual1, int le
         if (isAdapterDimer) { result1 = FAIL_ADAPTER_DIMER; result2 = FAIL_ADAPTER_DIMER; flags1 |= FP_F_ADAPTER_DIMER; flags2 |= FP_F_ADAPTER_DIMER; }
         pv = std::max(result1, result2);
         w.fr->addFilterResult(pv, 2);                                         // :573
-        if (!mOptions->merge.enabled && r1 != NULL && result1 == PASS_FILTER && r2 != NULL && result2 == PASS_FILTER) {   // :577-591
+        if (!dedupOut && !mOptions->merge.enabled && r1 != NULL && result1 == PASS_FILTER && r2 != NULL && result2 == PASS_FILTER) {   // :575-591
             w.post1->statRead(r1);
             w.post2->statRead(r2);
         }
@@ -353,16 +353,16 @@ void dump_worker(Worker& w, const fp_params* p, const fp_counter_layout* L, int6
 }
 
 void run_range(const fp_params* p, const fp_counter_layout* L, const fp_batch* b, int64_t lo, int64_t hi,
-               fp_read_result* out1, fp_read_result* out2, fp_ov_result* ov, int64_t* C) {
+               fp_read_result* out1, fp_read_result* out2, fp_ov_result* ov, int64_t* C, const uint8_t* is_dup = nullptr) {
     Worker w(p, L->cycles);
     fp_read_result tmp1, tmp2;
     for (int64_t i = lo; i < hi; i++) {
         if (p->paired)
             pe_one(w, p, b->seq1 + i * b->stride, b->qual1 + i * b->stride, b->len1[i],
-                   b->seq2 + i * b->stride, b->qual2 + i * b->stride, b->len2[i],
+                   b->seq2 + i * b->stride, b->qual2 + i * b->stride, b->len2[i], is_dup && is_dup[i],
                    out1 ? out1 + i : &tmp1, out2 ? out2 + i : &tmp2, ov ? ov + i : NULL);
         else
-            se_one(w, p, b->seq1 + i * b->stride, b->qual1 + i * b->stride, b->len1[i], out1 ? out1 + i : &tmp1);
+            se_one(w, p, b->seq1 + i * b->stride, b->qual1 + i * b->stride, b->len1[i], is_dup && is_dup[i], out1 ? out1 + i : &tmp1);
     }
     dump_worker(w, p, L, C);
 }
@@ -378,6 +378,13 @@ int fp_ref_process(const fp_params* p, const fp_counter_layout* L, const fp_batc
     return FP_OK;
 }
 
+// Same contract as fp_oracle_process_dedup: is_dup[i] is what `mDuplicate->checkPair(or1, or2) && mOptions->duplicate.dedup` gave for unit i.
+int fp_ref_process_dedup(const fp_params* p, const fp_counter_layout* L, const fp_batch* b, const uint8_t* is_dup,
+                         fp_read_result* out1, fp_read_result* out2, fp_ov_result* ov, int64_t* counters) {
+    run_range(p, L, b, 0, b->n, out1, out2, ov, counters, is_dup);
+    return FP_OK;
+}
+
 // Single worker over the whole batch + the reference's own adapter-string histograms (FilterResult::mAdapter1 / mAdapter2,
 // src/filterresult.cpp:124-180) serialised as "1\tSEQ\tCOUNT\n" / "2\t..." lines in map order.  Returns the number of lines.
 int fp_ref_process_maps(const fp_params* p, const fp_counter_layout* L, const fp_batch* b, int64_t* counters, char* out, int64_t cap, int64_t* used) {
@@ -385,9 +392,9 @@ int fp_ref_process_maps(const fp_params* p, const fp_counter_layout* L, const fp
     fp_read_result t1, t2;
     for (int64_t i = 0; i < b->n; i++) {
         if (p->paired)
-            pe_one(w, p, b->seq1 + i * b->stride, b->qual1 + i * b->stride, b->len1[i], b->seq2 + i * b->stride, b->qual2 + i * b->stride, b->len2[i], &t1, &t2, NULL);
+            pe_one(w, p, b->seq1 + i * b->stride, b->qual1 + i * b->stride, b->len1[i], b->seq2 + i * b->stride, b->qual2 + i * b->stride, b->len2[i], false, &t1, &t2, NULL);
         else
-            se_one(w, p, b->seq1 + i * b->stride, b->qual1 + i * b->stride, b->len1[i], &t1);
+            se_one(w, p, b->seq1 + i * b->stride, b->qual1 + i * b->stride, b->len1[i], false, &t1);
     }
     dump_worker(w, p, L, counters);
     std::string o; int n = 0;

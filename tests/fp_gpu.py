@@ -81,8 +81,10 @@ def pack_rows(lib, b, arrs, paired, threads=4):
     return pb, keep
 
 
-def run_gpu(params, arrs, cycles, mode="device", ctx=None, splits=1):
-    """Run the CUDA hot path over a COPY of arrs; same return shape as fp_testlib.run_cpu."""
+def run_gpu(params, arrs, cycles, mode="device", ctx=None, splits=1, is_dup=None):
+    """Run the CUDA hot path over a COPY of arrs; same return shape as fp_testlib.run_cpu.
+    is_dup (mode "device" only): --dedup flags of the units, uploaded and given to every launch through fp_set_dup_flags at that
+    launch's first unit, and cleared afterwards."""
     torch = _torch()
     paired = bool(params.paired)
     n, stride = arrs["seq1"].shape
@@ -104,8 +106,15 @@ def run_gpu(params, arrs, cycles, mode="device", ctx=None, splits=1):
             cap = 4 * n + 16
             d_patch = torch.zeros(cap * 12, dtype=torch.uint8, device="cuda:0")
             d_np = torch.zeros(1, dtype=torch.int32, device="cuda:0")
+        d_dup = None
+        if is_dup is not None:
+            flags = np.ascontiguousarray(is_dup, np.uint8)
+            assert flags.shape == (n,)
+            d_dup = torch.from_numpy(np.concatenate([flags, np.zeros(1, np.uint8)])).cuda()
         bounds = [n * i // splits for i in range(splits + 1)]
         for lo, hi in zip(bounds[:-1], bounds[1:]):          # consecutive sub-batches of one stream (counters accumulate)
+            if d_dup is not None:
+                capi.check(lib.fp_set_dup_flags(ctx.h, d_dup.data_ptr() + lo), lib)
             sb = capi.Batch()
             sb.n, sb.stride = hi - lo, stride
             for k, v in t.items():
@@ -117,6 +126,8 @@ def run_gpu(params, arrs, cycles, mode="device", ctx=None, splits=1):
             else:
                 capi.check(lib.fp_process_se(ctx.h, C.byref(sb), d_out1.data_ptr() + lo * 16, None), lib)
         torch.cuda.synchronize()
+        if d_dup is not None:
+            capi.check(lib.fp_set_dup_flags(ctx.h, None), lib)
         out1 = d_out1.cpu().numpy().view(capi.READ_RESULT_DTYPE)[:n].copy()
         if paired:
             out2 = d_out2.cpu().numpy().view(capi.READ_RESULT_DTYPE)[:n].copy()
@@ -126,6 +137,8 @@ def run_gpu(params, arrs, cycles, mode="device", ctx=None, splits=1):
         for k in a:
             a[k] = t[k].cpu().numpy()
         extra = {"patches": patches, "n_patches": npatch} if paired else {}
+    elif is_dup is not None:
+        raise ValueError("is_dup goes with mode='device': the host entry points refuse a set flag pointer")
     elif mode in ("host_tight", "host_tight_pack2bit"):
         # host rows at pitch = longest read (no padding bytes over PCIe); corrected rows come back at that pitch.
         # _pack2bit: FP_B_PACK2BIT, the library's host threads pack the bases chunk by chunk under the copies
@@ -175,13 +188,15 @@ def run_gpu(params, arrs, cycles, mode="device", ctx=None, splits=1):
 
 
 # ---------------- FASTQ text <-> rows ----------------
-def gpu_fastq_decode(ctx, text, final=1, phred64=0, capacity=None):
-    """fp_fastq_decode on cuda:0; same return shape as fp_testlib.oracle_fastq_decode (+ the device tensors)."""
+def gpu_fastq_decode(ctx, text, final=1, phred64=0, capacity=None, misalign=0):
+    """fp_fastq_decode on cuda:0; same return shape as fp_testlib.oracle_fastq_decode (+ the device tensors).
+    misalign: the text starts that many bytes behind a 256-byte aligned device address."""
     torch = _torch()
     lib = ctx.lib
     cap = capacity if capacity is not None else text.count(b"@") + 2
     cap1 = max(cap, 1)
-    d_text = torch.from_numpy(np.frombuffer(text, np.uint8).copy() if len(text) else np.zeros(1, np.uint8)).cuda()
+    d_text = torch.from_numpy(np.concatenate([np.zeros(misalign, np.uint8), np.frombuffer(text, np.uint8), np.zeros(1, np.uint8)])).cuda()[misalign:]
+    assert d_text.data_ptr() % 16 == misalign % 16
     d_seq = torch.full((cap1 * ctx.stride + 64,), 0xEE, dtype=torch.uint8, device="cuda:0")
     d_qual = torch.full((cap1 * ctx.stride + 64,), 0xEE, dtype=torch.uint8, device="cuda:0")
     d_len = torch.zeros(cap1, dtype=torch.int16, device="cuda:0")
@@ -213,20 +228,32 @@ def gpu_fastq_encode(ctx, dev, res, n):
     return d_out.cpu().numpy()[:total.value].tobytes()
 
 
-def gpu_fastq_process_host(ctx, text1, text2=None, final=1, phred64=0):
-    """fp_fastq_process_host: text in, filtered text out (host buffers)."""
+GUARD = 0xA5
+
+
+def gpu_fastq_process_host(ctx, text1, text2=None, final=1, phred64=0, out_cap=None):
+    """fp_fastq_process_host: text in, filtered text out (host buffers).  out_cap = (cap1, cap2) gives the output buffers exactly
+    that size, with 64 guard bytes behind them that must come back untouched ("guard_ok")."""
     lib = ctx.lib
-    b1 = np.frombuffer(text1, np.uint8).copy() if len(text1) else np.zeros(1, np.uint8)
-    o1 = np.zeros(len(text1) + 64, np.uint8); n1 = C.c_int64(); c1 = C.c_int64(); c2 = C.c_int64(); nu = C.c_int64()
-    i1, i2 = capi.FastqInfo(), capi.FastqInfo()
+    texts = [text1] + ([text2] if text2 is not None else [])
+    caps = list(out_cap) if out_cap is not None else [len(t) + 64 for t in texts]
+    bufs = [np.frombuffer(t, np.uint8).copy() if len(t) else np.zeros(1, np.uint8) for t in texts]
+    outs = [np.full(c + 64, GUARD, np.uint8) for c in caps]
+    nout = [C.c_int64(), C.c_int64()]; cons = [C.c_int64(), C.c_int64()]; nu = C.c_int64()
+    infos = [capi.FastqInfo(), capi.FastqInfo()]
     if text2 is not None:
-        b2 = np.frombuffer(text2, np.uint8).copy() if len(text2) else np.zeros(1, np.uint8)
-        o2 = np.zeros(len(text2) + 64, np.uint8); n2 = C.c_int64()
-        capi.check(lib.fp_fastq_process_host(ctx.h, b1.ctypes.data, len(text1), b2.ctypes.data, len(text2), final, phred64,
-                                             o1.ctypes.data, o1.size, C.byref(n1), o2.ctypes.data, o2.size, C.byref(n2),
-                                             C.byref(nu), C.byref(c1), C.byref(c2), C.byref(i1), C.byref(i2)), lib)
-        return {"out1": o1[:n1.value].tobytes(), "out2": o2[:n2.value].tobytes(), "n": nu.value, "consumed": (c1.value, c2.value)}
-    capi.check(lib.fp_fastq_process_host(ctx.h, b1.ctypes.data, len(text1), None, 0, final, phred64,
-                                         o1.ctypes.data, o1.size, C.byref(n1), None, 0, None,
-                                         C.byref(nu), C.byref(c1), None, C.byref(i1), None), lib)
-    return {"out1": o1[:n1.value].tobytes(), "n": nu.value, "consumed": (c1.value,)}
+        rc = lib.fp_fastq_process_host(ctx.h, bufs[0].ctypes.data, len(text1), bufs[1].ctypes.data, len(text2), final, phred64,
+                                       outs[0].ctypes.data, caps[0], C.byref(nout[0]), outs[1].ctypes.data, caps[1], C.byref(nout[1]),
+                                       C.byref(nu), C.byref(cons[0]), C.byref(cons[1]), C.byref(infos[0]), C.byref(infos[1]))
+    else:
+        rc = lib.fp_fastq_process_host(ctx.h, bufs[0].ctypes.data, len(text1), None, 0, final, phred64,
+                                       outs[0].ctypes.data, caps[0], C.byref(nout[0]), None, 0, None,
+                                       C.byref(nu), C.byref(cons[0]), None, C.byref(infos[0]), None)
+    guard_ok = all(bool((o[c:] == GUARD).all()) for o, c in zip(outs, caps))
+    if out_cap is None:
+        capi.check(rc, lib)
+    res = {"rc": rc, "guard_ok": guard_ok, "n": nu.value, "consumed": tuple(c.value for c in cons[:len(texts)]),
+           "info": [{k: int(getattr(i, k)) for k, _ in capi.FastqInfo._fields_} for i in infos[:len(texts)]]}
+    for k, (o, c, nb) in enumerate(zip(outs, caps, nout)):
+        res["out%d" % (k + 1)] = o[:min(nb.value, c)].tobytes() if rc == 0 else b""
+    return res

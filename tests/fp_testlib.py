@@ -19,6 +19,7 @@ TRUSEQ_R2 = "AGATCGGAAGAGCGTCGTGTAGGGAAAGAGTGT"
 
 _PROC_ARGS = [C.POINTER(capi.Params), C.POINTER(capi.CounterLayout), C.POINTER(capi.Batch),
               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+_DEDUP_ARGS = _PROC_ARGS[:3] + [C.c_void_p] + _PROC_ARGS[3:]          # + is_dup[n] after the batch
 
 _oracle = None
 _ref = None
@@ -37,6 +38,12 @@ def oracle():
         capi.bind(lib, ["fp_params_default", "fp_counter_layout_make", "fp_counter_layout_make_overrep", "fp_abi_sizeof"])
         lib.fp_oracle_process.restype = C.c_int
         lib.fp_oracle_process.argtypes = _PROC_ARGS
+        lib.fp_oracle_process_dedup.restype = C.c_int
+        lib.fp_oracle_process_dedup.argtypes = _DEDUP_ARGS
+        lib.fp_oracle_dup_create.restype = C.c_void_p; lib.fp_oracle_dup_create.argtypes = [C.c_int]
+        lib.fp_oracle_dup_check.argtypes = [C.c_void_p, C.POINTER(capi.Batch), C.c_int, C.c_void_p]
+        lib.fp_oracle_dup_totals.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        lib.fp_oracle_dup_destroy.argtypes = [C.c_void_p]
         lib.fp_synth_fill_host.restype = C.c_int
         lib.fp_synth_fill_host.argtypes = [C.POINTER(capi.Batch), C.c_int64, C.c_uint64, C.c_int32, C.c_int32]
         lib.fp_oracle_trim_and_cut.restype = C.c_int
@@ -78,6 +85,16 @@ def ref():
     return _ref
 
 
+def have_ref_dedup():
+    """oracle/_ref/libfastp_ref.so exports fp_ref_process_dedup.  A library built from an older oracle/ref_build/ref_harness.cpp
+    (one that travelled with the tree instead of being rebuilt) serves every other fp_ref_* entry point as before."""
+    if not have_ref() or not hasattr(ref(), "fp_ref_process_dedup"):
+        return False
+    ref().fp_ref_process_dedup.restype = C.c_int
+    ref().fp_ref_process_dedup.argtypes = _DEDUP_ARGS
+    return True
+
+
 def copy_arrays(arrs):
     return {k: v.copy() for k, v in arrs.items()}
 
@@ -89,8 +106,9 @@ def synth_host(n, stride, paired, first_index, seed, profile, read_len):
     return b, arrs
 
 
-def run_cpu(which, params, arrs, cycles, nthreads=0):
+def run_cpu(which, params, arrs, cycles, nthreads=0, is_dup=None):
     """Run the C port ('oracle') or the reference harness ('ref') over a COPY of arrs.
+    is_dup: per-unit --dedup flags (uint8[n]) as the duplicate filter gave them, None = --dedup off.
     Returns dict(out1, out2, ov, counters(CounterView), arrs(after correction))."""
     a = copy_arrays(arrs)
     b = capi.batch_from_arrays(a)
@@ -103,7 +121,13 @@ def run_cpu(which, params, arrs, cycles, nthreads=0):
     cnt = np.zeros(L.total, np.int64)
     args = (C.byref(params), C.byref(L), C.byref(b), out1.ctypes.data, out2.ctypes.data if paired else None,
             ov.ctypes.data if paired else None, cnt.ctypes.data)
-    if which == "oracle":
+    if is_dup is not None:
+        flags = np.ascontiguousarray(is_dup, np.uint8)
+        assert flags.shape == (n,) and not nthreads
+        assert which == "oracle" or have_ref_dedup(), "libfastp_ref.so has no fp_ref_process_dedup: rebuild it (make -C oracle)"
+        fn = oracle().fp_oracle_process_dedup if which == "oracle" else ref().fp_ref_process_dedup
+        rc = fn(*args[:3], flags.ctypes.data, *args[3:])
+    elif which == "oracle":
         rc = oracle().fp_oracle_process(*args)
     elif nthreads:
         rc = ref().fp_ref_process_mt(*args, nthreads)
@@ -367,9 +391,31 @@ def fastq_edge_cases():
     }
 
 
-def fastq_fuzz_text(rng, nrec=30):
+def oracle_dup_flags(batches, paired, level=1):
+    """The sequential duplicate filter (C port of Duplicate::checkRead / checkPair) over `batches` in order, one filter for all of
+    them: (list of uint8 flag arrays, total, dups)."""
+    lib = oracle()
+    d = lib.fp_oracle_dup_create(level)
+    assert d
+    try:
+        out = []
+        for arrs in batches:
+            a = {k: np.ascontiguousarray(v) for k, v in arrs.items()}
+            f = np.zeros(len(a["len1"]), np.uint8)
+            if len(f):
+                b = capi.batch_from_arrays(a)
+                lib.fp_oracle_dup_check(d, C.byref(b), paired, f.ctypes.data)
+            out.append(f)
+        t, k = C.c_int64(), C.c_int64()
+        lib.fp_oracle_dup_totals(d, C.byref(t), C.byref(k))
+        return out, t.value, k.value
+    finally:
+        lib.fp_oracle_dup_destroy(d)
+
+
+def fastq_fuzz_text(rng, nrec=30, broken=0.04):
     """Random FASTQ-ish text: mixed line ends, blank / junk lines between records, odd strand lines, empty reads,
-    occasional broken records, optional missing final terminator."""
+    occasional broken records (a share `broken` of them), optional missing final terminator."""
     eols = ["\n", "\r\n", "\r"]
     out = []
     for i in range(nrec):
@@ -383,15 +429,91 @@ def fastq_fuzz_text(rng, nrec=30):
             q = "@" + q[1:]
         strand = "+" if rng.random() < 0.8 else "+" + "x" * int(rng.integers(1, 9))
         r = rng.random()
-        if r < 0.02:
+        if r < broken / 2:
             strand = "-"                               # reader stops here
-        elif r < 0.04:
+        elif r < broken:
             q = q + "I"                                # length mismatch: reader stops here
         out.append(f"@r{i} {'y' * int(rng.integers(0, 20))}{e}{s}{e}{strand}{e}{q}{e}")
     text = "".join(out)
     if rng.random() < 0.3 and text:
         text = text.rstrip("\r\n")
     return text.encode()
+
+
+# ---------------- long dirty texts: the record automaton past one warp (256 lines) and one block (2 048 lines) ----------------
+FQ_LINES_PER_BLOCK = 2048                                   # FQ_LB of fastp_b200/csrc/fp_fastq.cuh
+FQ_BYTES_PER_BLOCK = 16384                                  # FQ_BB
+
+
+def fastq_shifted_text(nrec=12000, seed=1, every=531, at_quality_on_block_start=True):
+    """Clean records with 1-3 lines that start no record (blank, junk, a lone '+') put between records every `every` lines or so.  Each
+    insertion moves the following name lines by 1-3 lines, so the 8-line thread, 256-line warp and 2 048-line block borders fall in
+    every position of a record.  Where a quality line lands on a block's first line it is made to begin with '@'."""
+    rng = np.random.default_rng(seed)
+    lines, next_junk = [], every // 3
+    for i in range(nrec):
+        if len(lines) >= next_junk:
+            lines += [["", "junk line", "+", "#c", "\t"][int(rng.integers(0, 5))] for _ in range(int(rng.integers(1, 4)))]
+            next_junk = len(lines) + every + int(rng.integers(0, 64))
+        n = int(rng.integers(1, 61))
+        s = "".join(rng.choice(list("ACGTN"), n))
+        q = "".join(chr(int(x)) for x in rng.integers(35, 75, n))
+        if at_quality_on_block_start and (len(lines) + 3) % FQ_LINES_PER_BLOCK == 0:
+            q = "@" + q[1:]
+        lines += [f"@r{i} {'y' * int(rng.integers(0, 20))}", s, "+" if i % 5 else f"+r{i}", q]
+    return ("\n".join(lines) + "\n").encode()
+
+
+def line_starts(text):
+    """Offsets at which the lines of a '\\n'-terminated text begin."""
+    nl = np.flatnonzero(np.frombuffer(text, np.uint8) == 10)
+    return np.concatenate([[0], nl + 1])[: len(nl) + (0 if text.endswith(b"\n") else 1)]
+
+
+def states_at_block_starts(text, recs):
+    """Position in its record (0 = between records or on a name line, 1-3 = sequence / strand / quality line) of the first line of
+    every 2 048-line block, from the name offsets a decode reported."""
+    ls = line_starts(text)
+    name_line = np.searchsorted(ls, recs["name_off"].astype(np.int64))
+    out = []
+    for b in range(0, len(ls), FQ_LINES_PER_BLOCK):
+        k = np.searchsorted(name_line, b, side="right") - 1
+        d = b - int(name_line[k]) if k >= 0 else 4
+        out.append(d if d < 4 else 0)
+    return out
+
+
+def fastq_eol_text(eol, nrec=3000, seed=2, straddle=(63, FQ_BYTES_PER_BLOCK - 1, 3 * FQ_BYTES_PER_BLOCK - 1)):
+    """Records ending their lines with `eol`; names are padded so that a name line's terminator begins exactly at each offset in
+    `straddle` (with "\\r\\n" the pair then lies across a 64-byte thread border or a 16 KiB block border)."""
+    rng = np.random.default_rng(seed)
+    out, size, todo = [], 0, sorted(straddle)
+    for i in range(nrec):
+        name = f"@e{i}"
+        if todo and todo[0] - size < 400:
+            pad = todo.pop(0) - size - len(name)
+            assert pad >= 0
+            name += "p" * pad
+        n = int(rng.integers(0, 61))
+        s = "".join(rng.choice(list("ACGTN"), n)) if n else ""
+        q = "".join(chr(int(x)) for x in rng.integers(35, 75, n)) if n else ""
+        r = eol.join([name, s, "+", q]) + eol
+        out.append(r); size += len(r)
+    assert not todo
+    text = "".join(out).encode()
+    for o in straddle:
+        assert text[o:o + len(eol)] == eol.encode()
+    return text
+
+
+def fastq_break_record(text, recs, idx, how):
+    """`text` with record idx made unreadable: how = 'strand' (the '+' becomes '-') or 'length' (one quality byte more)."""
+    r = recs[idx]
+    if how == "strand":
+        o = int(r["strand_off"])
+        return text[:o] + b"-" + text[o + 1:]
+    o = text.index(b"\n", int(r["strand_off"])) + 1
+    return text[:o] + b"I" + text[o:]
 
 
 def random_params(rng, paired, lib=None):
