@@ -113,6 +113,7 @@ class FastqInfo(C.Structure):
 # name -> (restype, argtypes): every symbol include/fastp_b200.h declares
 FP_B_INDEXED = 0x1          # fp_batch.flags
 FP_B_PACK2BIT = 0x2
+FP_FQ_OUT_MERGED, FP_FQ_OUT_R1, FP_FQ_OUT_R2 = 0, 1, 2   # fp_fastq_encode_merge `which`
 
 SYMBOLS = {
     "fp_params_default": (None, [C.POINTER(Params), C.c_int]),
@@ -172,6 +173,12 @@ SYMBOLS = {
                                         C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p, C.c_int64, C.POINTER(C.c_int64),
                                         C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
                                         C.POINTER(FastqInfo), C.POINTER(FastqInfo)]),
+    "fp_fastq_encode_merge": (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 11 + [C.c_int64, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]),
+    "fp_fastq_process_host_merge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
+                                              C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p, C.c_int64, C.POINTER(C.c_int64),
+                                              C.c_void_p, C.c_int64, C.POINTER(C.c_int64),
+                                              C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                              C.POINTER(FastqInfo), C.POINTER(FastqInfo)]),
 }
 
 

@@ -109,7 +109,7 @@ struct fp_ctx {
     /* FASTQ codec workspaces (grown on demand) and the buffers of fp_fastq_process_host */
     struct Buf { void* p = nullptr; size_t cap = 0; };
     Buf fq_term, fq_bcnt, fq_agg, fq_bstate, fq_brec, fq_recline, fq_recend, fq_info, fq_bsum;
-    Buf fqh_text[2], fqh_seq[2], fqh_qual[2], fqh_len[2], fqh_recs[2], fqh_res[2], fqh_ov, fqh_out[2], fqh_outbuf[2][2], fqh_recend[2];
+    Buf fqh_text[2], fqh_seq[2], fqh_qual[2], fqh_len[2], fqh_recs[2], fqh_res[2], fqh_ov, fqh_out[2], fqh_outbuf[2][3], fqh_recend[2];
     unsigned int *fq_hinfo = nullptr, *fq_hinfo_dev = nullptr;      /* mapped pinned control words */
     cudaStream_t fq_stream_out = nullptr;
     cudaEvent_t fq_ev_up = nullptr, fq_ev_out[2] = {nullptr, nullptr};
@@ -462,7 +462,7 @@ extern "C" void fp_ctx_destroy(fp_ctx* c) {
         fp_ctx::Buf* all[] = {&c->fq_term, &c->fq_bcnt, &c->fq_agg, &c->fq_bstate, &c->fq_brec, &c->fq_recline, &c->fq_recend, &c->fq_info, &c->fq_bsum,
                               &c->fqh_text[0], &c->fqh_text[1], &c->fqh_seq[0], &c->fqh_seq[1], &c->fqh_qual[0], &c->fqh_qual[1], &c->fqh_len[0], &c->fqh_len[1],
                               &c->fqh_recs[0], &c->fqh_recs[1], &c->fqh_res[0], &c->fqh_res[1], &c->fqh_ov, &c->fqh_out[0], &c->fqh_out[1],
-                              &c->fqh_outbuf[0][0], &c->fqh_outbuf[0][1], &c->fqh_outbuf[1][0], &c->fqh_outbuf[1][1], &c->fqh_recend[0], &c->fqh_recend[1], &c->fq_dupflags};
+                              &c->fqh_outbuf[0][0], &c->fqh_outbuf[0][1], &c->fqh_outbuf[0][2], &c->fqh_outbuf[1][0], &c->fqh_outbuf[1][1], &c->fqh_outbuf[1][2], &c->fqh_recend[0], &c->fqh_recend[1], &c->fq_dupflags};
         if (c->dup.bits) cudaFree(c->dup.bits);
         cudaFree(c->d_dup_primes); cudaFree(c->d_dup_count);
         fq_free(c->dup_pos); fq_free(c->dup_keys); fq_free(c->dup_vals);
@@ -1368,37 +1368,67 @@ extern "C" int fp_fastq_decode(fp_ctx* c, const uint8_t* d_text, int64_t nbytes,
     return fastq_decode_impl(c, d_text, nbytes, final_chunk, phred64, d_seq, d_qual, d_len, capacity, d_recs, info, c->fq_recend);
 }
 
-extern "C" int fp_fastq_encode(fp_ctx* c, const uint8_t* d_text, const fp_fastq_rec* d_recs, const fp_read_result* d_res,
-                               const uint8_t* d_seq, const uint8_t* d_qual, int64_t n, uint8_t* d_out, int64_t out_cap, int64_t* out_bytes) {
-    if (!c || !out_bytes) return set_err(FP_E_INVAL, "null argument");
-    *out_bytes = 0;
-    if (n <= 0) return FP_OK;
-    if (!d_text || !d_recs || !d_res || !d_seq || !d_qual || (out_cap > 0 && !d_out)) return set_err(FP_E_INVAL, "null argument");
+/* size pass, scan and write pass of one output stream (fp_fastq.cuh); M is unused by FQ_SEL_PLAIN */
+template <int SEL>
+static int fastq_encode_impl(fp_ctx* c, const uint8_t* d_text, const fp_fastq_rec* d_recs, const fp_read_result* d_res,
+                             const uint8_t* d_seq, const uint8_t* d_qual, const fq_merge_args& M, int64_t n, uint8_t* d_out, int64_t out_cap, int64_t* out_bytes) {
     CK(cudaSetDevice(c->device));
     cudaStream_t st = c->stream[0];
     const int nblk = (int)((n + FQ_SCAN_ITEMS - 1) / FQ_SCAN_ITEMS);
     int rc;
     if ((rc = fq_ensure(c->fq_bsum, (size_t)(nblk + 1) * 8))) return rc;
     unsigned long long* d_bs = (unsigned long long*)c->fq_bsum.p;
-    fq_size_blocksum_kernel<<<nblk, FQ_T, 0, st>>>(reinterpret_cast<const fq_rec*>(d_recs), d_res, n, d_bs);
+    fq_size_blocksum_kernel<SEL><<<nblk, FQ_T, 0, st>>>(d_text, reinterpret_cast<const fq_rec*>(d_recs), d_res, M, n, d_bs);
     if (!c->fq_hinfo) { CK(cudaHostAlloc((void**)&c->fq_hinfo, 256, cudaHostAllocMapped)); CK(cudaHostGetDevicePointer((void**)&c->fq_hinfo_dev, c->fq_hinfo, 0)); }
     fq_size_scan_kernel<<<1, 32, 0, st>>>(d_bs, nblk, reinterpret_cast<unsigned long long*>(c->fq_hinfo_dev + 32));
-    fq_encode_kernel<<<nblk, FQ_T, 0, st>>>(d_text, reinterpret_cast<const fq_rec*>(d_recs), d_res, d_seq, d_qual, c->stride, n, d_bs, d_out,
-                                            (unsigned long long)std::max<int64_t>(out_cap, 0));
+    fq_encode_kernel<SEL><<<nblk, FQ_T, 0, st>>>(d_text, reinterpret_cast<const fq_rec*>(d_recs), d_res, d_seq, d_qual, M, c->stride, n, d_bs, d_out,
+                                                 (unsigned long long)std::max<int64_t>(out_cap, 0));
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(st));
     *out_bytes = (int64_t)*reinterpret_cast<volatile unsigned long long*>(c->fq_hinfo + 32);
     return FP_OK;
 }
 
-extern "C" int fp_fastq_process_host(fp_ctx* c, const uint8_t* text1, int64_t nbytes1, const uint8_t* text2, int64_t nbytes2,
-                                     int32_t final_chunk, int32_t phred64,
-                                     uint8_t* out1, int64_t out_cap1, int64_t* out_bytes1,
-                                     uint8_t* out2, int64_t out_cap2, int64_t* out_bytes2,
-                                     int64_t* n_units, int64_t* consumed1, int64_t* consumed2, fp_fastq_info* info1, fp_fastq_info* info2) {
-    if (!c || !n_units || !consumed1 || !out_bytes1) return set_err(FP_E_INVAL, "null argument");
+extern "C" int fp_fastq_encode(fp_ctx* c, const uint8_t* d_text, const fp_fastq_rec* d_recs, const fp_read_result* d_res,
+                               const uint8_t* d_seq, const uint8_t* d_qual, int64_t n, uint8_t* d_out, int64_t out_cap, int64_t* out_bytes) {
+    if (!c || !out_bytes) return set_err(FP_E_INVAL, "null argument");
+    *out_bytes = 0;
+    if (n <= 0) return FP_OK;
+    if (!d_text || !d_recs || !d_res || !d_seq || !d_qual || (out_cap > 0 && !d_out)) return set_err(FP_E_INVAL, "null argument");
+    return fastq_encode_impl<FQ_SEL_PLAIN>(c, d_text, d_recs, d_res, d_seq, d_qual, fq_merge_args{}, n, d_out, out_cap, out_bytes);
+}
+
+extern "C" int fp_fastq_encode_merge(fp_ctx* c, int32_t which, const uint8_t* d_text1, const fp_fastq_rec* d_recs1, const uint8_t* d_text2, const fp_fastq_rec* d_recs2,
+                                     const fp_read_result* d_res1, const fp_read_result* d_res2, const fp_ov_result* d_ov,
+                                     const uint8_t* d_seq1, const uint8_t* d_qual1, const uint8_t* d_seq2, const uint8_t* d_qual2,
+                                     int64_t n, uint8_t* d_out, int64_t out_cap, int64_t* out_bytes) {
+    if (!c || !out_bytes) return set_err(FP_E_INVAL, "null argument");
+    *out_bytes = 0;
+    if (!c->p.paired) return set_err(FP_E_INVAL, "ctx was created for single-end data: merging needs pairs");
+    if (!c->p.merge_enabled) return set_err(FP_E_INVAL, "ctx was created without merge_enabled (fp_fastq_encode writes its output)");
+    if (which != FP_FQ_OUT_MERGED && which != FP_FQ_OUT_R1 && which != FP_FQ_OUT_R2) return set_err(FP_E_INVAL, "which must be FP_FQ_OUT_MERGED, FP_FQ_OUT_R1 or FP_FQ_OUT_R2");
+    if (n <= 0) return FP_OK;
+    if (!d_text1 || !d_recs1 || !d_text2 || !d_recs2 || !d_res1 || !d_res2 || !d_ov || !d_seq1 || !d_qual1 || !d_seq2 || !d_qual2 || (out_cap > 0 && !d_out))
+        return set_err(FP_E_INVAL, "null argument");
+    fq_merge_args M{};
+    M.ov = d_ov; M.include_unmerged = c->p.merge_include_unmerged ? 1 : 0;
+    if (which == FP_FQ_OUT_R2) {                                  /* side 2 is written, side 1 only gives its records */
+        M.res2 = d_res1;
+        return fastq_encode_impl<FQ_SEL_SIDE>(c, d_text2, d_recs2, d_res2, d_seq2, d_qual2, M, n, d_out, out_cap, out_bytes);
+    }
+    M.text2 = d_text2; M.recs2 = reinterpret_cast<const fq_rec*>(d_recs2); M.res2 = d_res2; M.seq2 = d_seq2; M.qual2 = d_qual2;
+    if (which == FP_FQ_OUT_R1) return fastq_encode_impl<FQ_SEL_SIDE>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
+    return fastq_encode_impl<FQ_SEL_MERGED>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
+}
+
+/* The round loop of the text path.  merging: the ctx merges pairs, so every round also keeps the chain's overlap results and encodes a
+   third stream (outs[2] = --merged_out) beside the two sides. */
+static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbytes1, const uint8_t* text2, int64_t nbytes2,
+                                   int32_t final_chunk, int32_t phred64, uint8_t* const outs[3], const int64_t ocap[3], int64_t* const out_bytes[3],
+                                   int64_t* n_units, int64_t* consumed1, int64_t* consumed2, fp_fastq_info* info1, fp_fastq_info* info2) {
     const int sides = c->p.paired ? 2 : 1;
-    if (sides == 2 && (!consumed2 || !out_bytes2)) return set_err(FP_E_INVAL, "paired ctx needs the second side");
+    const bool merging = c->p.merge_enabled && sides == 2;
+    const int nstreams = merging ? 3 : sides;
     if (c->dup_flags) return set_err(FP_E_INVAL, "duplicate flags are set (fp_set_dup_flags): the text path runs its own duplicate filter (fp_fastq_set_dedup)");
     CK(cudaSetDevice(c->device));
     cudaStream_t st = c->stream[0], up = c->stream[1];
@@ -1410,7 +1440,6 @@ extern "C" int fp_fastq_process_host(fp_ctx* c, const uint8_t* text1, int64_t nb
     cudaStream_t outst = c->fq_stream_out;
     const uint8_t* text[2] = {text1, text2};
     const int64_t nb[2] = {nbytes1, sides == 2 ? nbytes2 : 0};
-    uint8_t* outs[2] = {out1, out2}; const int64_t ocap[2] = {out_cap1, out_cap2};
     const int64_t cap = c->max_batch;
     /* The text goes up in pieces on its own stream while the pieces already on the device are decoded, run through the chain and
        encoded, and the previous round's output text goes down on a third stream: H2D, kernels and D2H overlap inside ONE call
@@ -1426,7 +1455,8 @@ extern "C" int fp_fastq_process_host(fp_ctx* c, const uint8_t* text1, int64_t nb
         if ((rc = fq_ensure(c->fqh_recs[s], (size_t)cap * sizeof(fp_fastq_rec)))) return rc;
         if ((rc = fq_ensure(c->fqh_res[s], (size_t)cap * sizeof(fp_read_result)))) return rc;
     }
-    int64_t upl[2] = {0, 0}, start[2] = {0, 0}, obytes[2] = {0, 0}, units = 0;
+    if (merging && (rc = fq_ensure(c->fqh_ov, (size_t)cap * sizeof(fp_ov_result)))) return rc;
+    int64_t upl[2] = {0, 0}, start[2] = {0, 0}, obytes[3] = {0, 0, 0}, units = 0;
     fp_fastq_info agg[2]; memset(agg, 0, sizeof(agg)); agg[0].error_record = agg[1].error_record = -1;
     int flip = 0;
     auto upload_more = [&]() -> int {
@@ -1489,20 +1519,30 @@ extern "C" int fp_fastq_process_host(fp_ctx* c, const uint8_t* text1, int64_t nb
             }
             struct FlagsBack { fp_ctx* c; const uint8_t* f; ~FlagsBack() { c->dup_flags = f; } } flags_back{c, saved_flags};
             if (sides == 2) {
-                rc = launch_chain(c, &b, (fp_read_result*)c->fqh_res[0].p, (fp_read_result*)c->fqh_res[1].p, nullptr, nullptr, 0, nullptr, st);
+                rc = launch_chain(c, &b, (fp_read_result*)c->fqh_res[0].p, (fp_read_result*)c->fqh_res[1].p, merging ? (fp_ov_result*)c->fqh_ov.p : nullptr,
+                                  nullptr, 0, nullptr, st);
             } else rc = launch_chain(c, &b, (fp_read_result*)c->fqh_res[0].p, nullptr, nullptr, nullptr, 0, nullptr, st);
             if (rc) return rc;
             CK(cudaEventSynchronize(c->fq_ev_out[flip]));        /* the output buffers of two rounds ago have gone down */
-            for (int s = 0; s < sides; s++) {
-                if (!outs[s]) continue;                           /* caller does not want this side's text */
+            const uint8_t* rtext[2] = {(const uint8_t*)c->fqh_text[0].p + rstart[0], sides == 2 ? (const uint8_t*)c->fqh_text[1].p + rstart[1] : nullptr};
+            for (int s = 0; s < nstreams; s++) {
+                if (!outs[s]) continue;                           /* caller does not want this stream's text */
                 fp_ctx::Buf& ob = c->fqh_outbuf[flip][s];
                 const int64_t room = std::max<int64_t>(ocap[s] - obytes[s], 0);
-                int64_t want = std::min<int64_t>(room, n * (int64_t)(2 * c->stride + 256));
+                /* per unit: one record of a side; on the merged stream one read of up to two rows, or two records */
+                int64_t want = std::min<int64_t>(room, n * (int64_t)(s == 2 ? 4 * c->stride + 512 : 2 * c->stride + 256));
                 int64_t total = 0;
                 for (int attempt = 0; attempt < 2; attempt++) {   /* names longer than the estimate: encode again into a buffer of the exact size */
                     if ((rc = fq_ensure(ob, (size_t)want + 64))) return rc;
-                    rc = fp_fastq_encode(c, (const uint8_t*)c->fqh_text[s].p + rstart[s], (const fp_fastq_rec*)c->fqh_recs[s].p, (const fp_read_result*)c->fqh_res[s].p,
-                                         (const uint8_t*)c->fqh_seq[s].p, (const uint8_t*)c->fqh_qual[s].p, n, (uint8_t*)ob.p, want, &total);
+                    if (merging)
+                        rc = fp_fastq_encode_merge(c, s == 2 ? FP_FQ_OUT_MERGED : s == 0 ? FP_FQ_OUT_R1 : FP_FQ_OUT_R2,
+                                                   rtext[0], (const fp_fastq_rec*)c->fqh_recs[0].p, rtext[1], (const fp_fastq_rec*)c->fqh_recs[1].p,
+                                                   (const fp_read_result*)c->fqh_res[0].p, (const fp_read_result*)c->fqh_res[1].p, (const fp_ov_result*)c->fqh_ov.p,
+                                                   (const uint8_t*)c->fqh_seq[0].p, (const uint8_t*)c->fqh_qual[0].p, (const uint8_t*)c->fqh_seq[1].p,
+                                                   (const uint8_t*)c->fqh_qual[1].p, n, (uint8_t*)ob.p, want, &total);
+                    else
+                        rc = fp_fastq_encode(c, rtext[s], (const fp_fastq_rec*)c->fqh_recs[s].p, (const fp_read_result*)c->fqh_res[s].p,
+                                             (const uint8_t*)c->fqh_seq[s].p, (const uint8_t*)c->fqh_qual[s].p, n, (uint8_t*)ob.p, want, &total);
                     if (rc) return rc;
                     if (total <= want) break;
                     if (total > room) return set_err(FP_E_TOOLARGE, "output buffer too small for the encoded FASTQ text");
@@ -1526,10 +1566,37 @@ extern "C" int fp_fastq_process_host(fp_ctx* c, const uint8_t* text1, int64_t nb
     if (trace) fprintf(stderr, "[fq] loop %.2f ms, drain %.2f ms\n", t_loop - t_begin, now() - t_loop);
     agg[0].consumed = start[0]; agg[1].consumed = start[1];
     *n_units = units; *consumed1 = start[0]; if (consumed2) *consumed2 = start[1];
-    *out_bytes1 = obytes[0]; if (out_bytes2) *out_bytes2 = obytes[1];
+    for (int s = 0; s < 3; s++) if (out_bytes[s]) *out_bytes[s] = obytes[s];
     if (info1) *info1 = agg[0];
     if (info2 && sides == 2) *info2 = agg[1];
     return FP_OK;
+}
+
+extern "C" int fp_fastq_process_host(fp_ctx* c, const uint8_t* text1, int64_t nbytes1, const uint8_t* text2, int64_t nbytes2,
+                                     int32_t final_chunk, int32_t phred64,
+                                     uint8_t* out1, int64_t out_cap1, int64_t* out_bytes1,
+                                     uint8_t* out2, int64_t out_cap2, int64_t* out_bytes2,
+                                     int64_t* n_units, int64_t* consumed1, int64_t* consumed2, fp_fastq_info* info1, fp_fastq_info* info2) {
+    if (!c || !n_units || !consumed1 || !out_bytes1) return set_err(FP_E_INVAL, "null argument");
+    if (c->p.paired && (!consumed2 || !out_bytes2)) return set_err(FP_E_INVAL, "paired ctx needs the second side");
+    if (c->p.paired && c->p.merge_enabled) return set_err(FP_E_INVAL, "ctx merges pairs: use fp_fastq_process_host_merge, which also returns the merged reads");
+    uint8_t* const outs[3] = {out1, out2, nullptr}; const int64_t ocap[3] = {out_cap1, out_cap2, 0};
+    int64_t* const ob[3] = {out_bytes1, out_bytes2, nullptr};
+    return fastq_process_host_impl(c, text1, nbytes1, text2, nbytes2, final_chunk, phred64, outs, ocap, ob, n_units, consumed1, consumed2, info1, info2);
+}
+
+extern "C" int fp_fastq_process_host_merge(fp_ctx* c, const uint8_t* text1, int64_t nbytes1, const uint8_t* text2, int64_t nbytes2,
+                                           int32_t final_chunk, int32_t phred64,
+                                           uint8_t* out1, int64_t out_cap1, int64_t* out_bytes1,
+                                           uint8_t* out2, int64_t out_cap2, int64_t* out_bytes2,
+                                           uint8_t* merged, int64_t merged_cap, int64_t* merged_bytes,
+                                           int64_t* n_units, int64_t* consumed1, int64_t* consumed2, fp_fastq_info* info1, fp_fastq_info* info2) {
+    if (!c || !n_units || !consumed1 || !consumed2 || !out_bytes1 || !out_bytes2 || !merged_bytes) return set_err(FP_E_INVAL, "null argument");
+    if (!c->p.paired) return set_err(FP_E_INVAL, "ctx was created for single-end data: merging needs pairs");
+    if (!c->p.merge_enabled) return set_err(FP_E_INVAL, "ctx was created without merge_enabled: use fp_fastq_process_host");
+    uint8_t* const outs[3] = {out1, out2, merged}; const int64_t ocap[3] = {out_cap1, out_cap2, merged_cap};
+    int64_t* const ob[3] = {out_bytes1, out_bytes2, merged_bytes};
+    return fastq_process_host_impl(c, text1, nbytes1, text2, nbytes2, final_chunk, phred64, outs, ocap, ob, n_units, consumed1, consumed2, info1, info2);
 }
 
 /* ---------------- duplication bloom filter (fp_dup.h / fp_dup.cuh) ---------------- */

@@ -305,15 +305,125 @@ __global__ void fq_finish_kernel(const unsigned int* term, unsigned int nlines, 
 __global__ void fq_set_u32_kernel(unsigned int* p, unsigned int v) { if (!blockIdx.x && !threadIdx.x) *p = v; }
 __global__ void fq_copy_u32_kernel(const unsigned int* src, unsigned int* dst) { if (!blockIdx.x && !threadIdx.x) *dst = *src; }
 
-/* ---- encode ---- */
+/* ---- encode ----
+ * One size pass, one scan and one write pass serve four output streams, chosen at compile time:
+ *   FQ_SEL_PLAIN   every unit whose pair verdict passes and that --dedup did not flag (peprocessor.cpp:575-584, seprocessor.cpp:268)
+ *   FQ_SEL_MERGED  --merged_out: the merged read of a merged pair (peprocessor.cpp:528-534; the duplicate flag is not consulted),
+ *                  or with --include_unmerged read 1 then read 2 of a pair that did not merge, each by its own verdict (:537-556)
+ *   FQ_SEL_SIDE    --out1 / --out2 in merging mode: only units that took neither merging branch (:563-585)
+ * The primary arrays (text, recs, res, seq, qual) are read 1's for FQ_SEL_MERGED and the written side's for FQ_SEL_SIDE;
+ * fq_merge_args carries the other side (FQ_SEL_SIDE reads only its records). */
 #define FQ_SCAN_ITEMS 2048
-__global__ void __launch_bounds__(FQ_T) fq_size_blocksum_kernel(const fq_rec* recs, const fp_read_result* res, long long n, unsigned long long* blocksum) {
+#define FQ_SEL_PLAIN 0
+#define FQ_SEL_MERGED 1
+#define FQ_SEL_SIDE 2
+struct fq_merge_args {
+    const uint8_t* text2; const fq_rec* recs2; const fp_read_result* res2; const uint8_t* seq2; const uint8_t* qual2;
+    const fp_ov_result* ov;
+    int include_unmerged;
+};
+/* which branch of peprocessor.cpp:519-622 a unit took, from its two records */
+#define FQ_U_ORDINARY 0
+#define FQ_U_MERGED 1
+#define FQ_U_UNMERGED 2
+__device__ __forceinline__ int fq_unit_class(const fp_read_result& a, const fp_read_result& b, int include_unmerged) {
+    if (a.flags & FP_F_MERGED) return FQ_U_MERGED;                                               /* :525 */
+    if (include_unmerged && !((a.flags | b.flags) & FP_F_DROPPED)) return FQ_U_UNMERGED;         /* :521 r1 && r2, :537 */
+    return FQ_U_ORDINARY;
+}
+__device__ __forceinline__ bool fq_written(const fp_read_result& r, unsigned int verdict) { return verdict == FP_PASS_FILTER && !(r.flags & FP_F_DUPLICATE); }
+__device__ __forceinline__ unsigned long long fq_record_size(const fq_rec& rc, const fp_read_result& r) {
+    return (unsigned long long)(rc.name_len & 0x0FFFFFFFu) + rc.strand_len + 2ull * r.len + 4ull;
+}
+__device__ __forceinline__ unsigned int fq_digits(unsigned int v) { return v < 10u ? 1u : v < 100u ? 2u : v < 1000u ? 3u : v < 10000u ? 4u : 5u; }
+/* " merged_<len1>_<len2>" (overlapanalysis.cpp:171): its length, and its byte t */
+__device__ __forceinline__ unsigned int fq_suffix_len(unsigned int len1, unsigned int len2) { return 9u + fq_digits(len1) + fq_digits(len2); }
+__device__ __forceinline__ uint8_t fq_suffix_byte(unsigned int t, unsigned int len1, unsigned int len2) {
+    if (t < 8u) return (uint8_t)" merged_"[t];
+    const unsigned int d1 = fq_digits(len1);
+    unsigned int v, k;                                          /* digit k (from the right) of v */
+    if (t < 8u + d1) { v = len1; k = 8u + d1 - 1u - t; }
+    else if (t == 8u + d1) return '_';
+    else { v = len2; k = 8u + d1 + fq_digits(len2) - t; }
+    for (; k > 0; k--) v /= 10u;
+    return (uint8_t)('0' + v % 10u);
+}
+/* fp_merged_lens for device code */
+__device__ __forceinline__ void fq_merged_lens(const fp_ov_result& ov, int r2_len, int& len1, int& len2) {
+    len1 = ov.overlap_len + (ov.offset > 0 ? ov.offset : 0);
+    len2 = ov.offset > 0 ? r2_len - ov.overlap_len : 0;
+}
+__device__ __forceinline__ bool fq_strand_is_plus(const uint8_t* text, const fq_rec& rc) { return rc.strand_len == 1 && text[rc.strand_off] == '+'; }
+/* bytes unit i puts on the selected stream */
+template <int SEL>
+__device__ __forceinline__ unsigned long long fq_unit_size(const uint8_t* text, const fq_rec* recs, const fp_read_result* res, const fq_merge_args& M, long long i) {
+    const fp_read_result r = res[i];
+    if (SEL == FQ_SEL_PLAIN) return fq_written(r, r.pair_verdict) ? fq_record_size(recs[i], r) : 0ull;
+    const fp_read_result r2 = M.res2[i];
+    const int cls = fq_unit_class(r, r2, M.include_unmerged);
+    if (SEL == FQ_SEL_SIDE) return cls == FQ_U_ORDINARY && fq_written(r, r.pair_verdict) ? fq_record_size(recs[i], r) : 0ull;
+    if (cls == FQ_U_MERGED) {
+        if (r.verdict != FP_PASS_FILTER) return 0ull;
+        int len1, len2;
+        fq_merged_lens(M.ov[i], r2.len, len1, len2);
+        const fq_rec rc = recs[i];
+        const unsigned int suf = fq_suffix_len((unsigned int)len1, (unsigned int)len2);
+        return (unsigned long long)(rc.name_len & 0x0FFFFFFFu) + suf + rc.strand_len + (fq_strand_is_plus(text, rc) ? 0u : suf) + 2ull * (unsigned int)(len1 + len2) + 4ull;
+    }
+    if (cls == FQ_U_UNMERGED) return (fq_written(r, r.verdict) ? fq_record_size(recs[i], r) : 0ull) + (fq_written(r2, r2.verdict) ? fq_record_size(M.recs2[i], r2) : 0ull);
+    return 0ull;
+}
+/* Read::appendToString (read.cpp:119-134) by one warp: name, kept window of the row, strand line, kept window of the qualities */
+__device__ __forceinline__ void fq_write_record(uint8_t* d, const uint8_t* text, const fq_rec& rc, const fp_read_result& rr,
+                                                const uint8_t* srow, const uint8_t* qrow, int lane) {
+    const unsigned int nl = rc.name_len & 0x0FFFFFFFu;
+    for (unsigned int t = lane; t < nl; t += 32) d[t] = text[rc.name_off + t];
+    if (lane == 0) d[nl] = '\n';
+    d += nl + 1;
+    for (unsigned int t = lane; t < rr.len; t += 32) d[t] = srow[rr.front + t];
+    if (lane == 0) d[rr.len] = '\n';
+    d += rr.len + 1;
+    for (unsigned int t = lane; t < rc.strand_len; t += 32) d[t] = text[rc.strand_off + t];
+    if (lane == 0) d[rc.strand_len] = '\n';
+    d += rc.strand_len + 1;
+    for (unsigned int t = lane; t < rr.len; t += 32) d[t] = qrow[rr.front + t];
+    if (lane == 0) d[rr.len] = '\n';
+}
+/* OverlapAnalysis::merge (overlapanalysis.cpp:148-179) by one warp: r1[0, len1) + reverse complement of r2[0, len2), qualities alike;
+ * the suffix goes on the name line and, unless it is exactly "+", on the strand line (:173-175).  Lane t of the reversed part reads
+ * s2[len2 - 1 - t]: consecutive lanes, consecutive addresses.  dev_complement is the reference's scalar map (simd.cpp:296-308). */
+__device__ __forceinline__ void fq_write_merged(uint8_t* d, const uint8_t* text, const fq_rec& rc, bool plus, unsigned int len1, unsigned int len2,
+                                                const uint8_t* s1, const uint8_t* q1, const uint8_t* s2, const uint8_t* q2, int lane) {
+    const unsigned int nl = rc.name_len & 0x0FFFFFFFu, suf = fq_suffix_len(len1, len2);
+    for (unsigned int t = lane; t < nl; t += 32) d[t] = text[rc.name_off + t];
+    d += nl;
+    for (unsigned int t = lane; t < suf; t += 32) d[t] = fq_suffix_byte(t, len1, len2);
+    if (lane == 0) d[suf] = '\n';
+    d += suf + 1;
+    for (unsigned int t = lane; t < len1; t += 32) d[t] = s1[t];
+    d += len1;
+    for (unsigned int t = lane; t < len2; t += 32) d[t] = dev_complement(s2[len2 - 1 - t]);
+    if (lane == 0) d[len2] = '\n';
+    d += len2 + 1;
+    for (unsigned int t = lane; t < rc.strand_len; t += 32) d[t] = text[rc.strand_off + t];
+    d += rc.strand_len;
+    if (!plus) { for (unsigned int t = lane; t < suf; t += 32) d[t] = fq_suffix_byte(t, len1, len2); d += suf; }
+    if (lane == 0) d[0] = '\n';
+    d += 1;
+    for (unsigned int t = lane; t < len1; t += 32) d[t] = q1[t];
+    d += len1;
+    for (unsigned int t = lane; t < len2; t += 32) d[t] = q2[len2 - 1 - t];
+    if (lane == 0) d[len2] = '\n';
+}
+template <int SEL>
+__global__ void __launch_bounds__(FQ_T) fq_size_blocksum_kernel(const uint8_t* text, const fq_rec* recs, const fp_read_result* res, fq_merge_args M,
+                                                                long long n, unsigned long long* blocksum) {
     __shared__ unsigned long long s[FQ_T / 32];
     const long long b0 = (long long)blockIdx.x * FQ_SCAN_ITEMS;
     unsigned long long c = 0;
     for (int k = threadIdx.x; k < FQ_SCAN_ITEMS; k += FQ_T) {
         const long long i = b0 + k;
-        if (i < n && res[i].pair_verdict == FP_PASS_FILTER && !(res[i].flags & FP_F_DUPLICATE)) c += (unsigned long long)(recs[i].name_len & 0x0FFFFFFFu) + recs[i].strand_len + 2ull * res[i].len + 4ull;
+        if (i < n) c += fq_unit_size<SEL>(text, recs, res, M, i);
     }
     #pragma unroll
     for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(FULL_MASK, c, o);
@@ -327,9 +437,10 @@ __global__ void fq_size_scan_kernel(unsigned long long* blocksum, int nblocks, u
     for (int i = 0; i < nblocks; i++) { const unsigned long long v = blocksum[i]; blocksum[i] = run; run += v; }
     *total = run;
 }
-/* one warp per record, FQ_SCAN_ITEMS records per block in order: the block's warps walk the records 8 at a time */
+/* one warp per unit, FQ_SCAN_ITEMS units per block in order: the block's warps walk the units 8 at a time */
+template <int SEL>
 __global__ void __launch_bounds__(FQ_T) fq_encode_kernel(const uint8_t* text, const fq_rec* recs, const fp_read_result* res,
-                                                         const uint8_t* seq, const uint8_t* qual, int stride, long long n,
+                                                         const uint8_t* seq, const uint8_t* qual, fq_merge_args M, int stride, long long n,
                                                          const unsigned long long* blockoff, uint8_t* out, unsigned long long out_cap) {
     __shared__ unsigned long long s_run;
     __shared__ unsigned long long s_sz[FQ_T];
@@ -338,10 +449,9 @@ __global__ void __launch_bounds__(FQ_T) fq_encode_kernel(const uint8_t* text, co
     __syncthreads();
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     for (int k0 = 0; k0 < FQ_SCAN_ITEMS; k0 += FQ_T) {
-        /* sizes of 256 consecutive records, exclusive scan inside the block */
+        /* sizes of 256 consecutive units, exclusive scan inside the block */
         const long long i = b0 + k0 + threadIdx.x;
-        unsigned long long sz = 0;
-        if (i < n && res[i].pair_verdict == FP_PASS_FILTER && !(res[i].flags & FP_F_DUPLICATE)) sz = (unsigned long long)(recs[i].name_len & 0x0FFFFFFFu) + recs[i].strand_len + 2ull * res[i].len + 4ull;
+        const unsigned long long sz = i < n ? fq_unit_size<SEL>(text, recs, res, M, i) : 0ull;
         unsigned long long inc = sz;
         #pragma unroll
         for (int o = 1; o < 32; o <<= 1) { const unsigned long long t = __shfl_up_sync(FULL_MASK, inc, o); if (lane >= o) inc += t; }
@@ -350,33 +460,33 @@ __global__ void __launch_bounds__(FQ_T) fq_encode_kernel(const uint8_t* text, co
         __syncthreads();
         unsigned long long before = s_run;
         for (int k = 0; k < w; k++) before += s_w[k];
-        s_sz[threadIdx.x] = before + inc - sz;                       /* output offset of record i */
+        s_sz[threadIdx.x] = before + inc - sz;                       /* output offset of unit i */
         __syncthreads();
-        /* copies: warp w takes records w, w+8, ... of this group */
+        /* copies: warp w takes units w, w+8, ... of this group */
         for (int j = w; j < FQ_T; j += FQ_T / 32) {
             const long long ri = b0 + k0 + j;
             if (ri >= n) break;
-            const fp_read_result rr = res[ri];
-            if (rr.pair_verdict != FP_PASS_FILTER || (rr.flags & FP_F_DUPLICATE)) continue;
-            const fq_rec rc = recs[ri];
-            const unsigned int nl = rc.name_len & 0x0FFFFFFFu;
-            unsigned long long o = s_sz[j];
-            const unsigned long long need = (unsigned long long)nl + rc.strand_len + 2ull * rr.len + 4ull;
-            if (o + need > out_cap) continue;                         /* caller sees total > cap */
+            const unsigned long long need = fq_unit_size<SEL>(text, recs, res, M, ri);
+            const unsigned long long o = s_sz[j];
+            if (need == 0 || o + need > out_cap) continue;            /* a unit that does not fit is skipped whole: caller sees total > cap */
             uint8_t* d = out + o;
-            for (unsigned int t = lane; t < nl; t += 32) d[t] = text[rc.name_off + t];
-            if (lane == 0) d[nl] = '\n';
-            d += nl + 1;
-            const uint8_t* srow = seq + (size_t)ri * stride + rr.front;
-            for (unsigned int t = lane; t < rr.len; t += 32) d[t] = srow[t];
-            if (lane == 0) d[rr.len] = '\n';
-            d += rr.len + 1;
-            for (unsigned int t = lane; t < rc.strand_len; t += 32) d[t] = text[rc.strand_off + t];
-            if (lane == 0) d[rc.strand_len] = '\n';
-            d += rc.strand_len + 1;
-            const uint8_t* qrow = qual + (size_t)ri * stride + rr.front;
-            for (unsigned int t = lane; t < rr.len; t += 32) d[t] = qrow[t];
-            if (lane == 0) d[rr.len] = '\n';
+            const fp_read_result rr = res[ri];
+            const fq_rec rc = recs[ri];
+            const uint8_t* srow = seq + (size_t)ri * stride;
+            const uint8_t* qrow = qual + (size_t)ri * stride;
+            if (SEL != FQ_SEL_MERGED) { fq_write_record(d, text, rc, rr, srow, qrow, lane); continue; }
+            const fp_read_result r2 = M.res2[ri];
+            const uint8_t* srow2 = M.seq2 + (size_t)ri * stride;
+            const uint8_t* qrow2 = M.qual2 + (size_t)ri * stride;
+            if (rr.flags & FP_F_MERGED) {
+                int len1, len2;
+                fq_merged_lens(M.ov[ri], r2.len, len1, len2);
+                fq_write_merged(d, text, rc, fq_strand_is_plus(text, rc), (unsigned int)len1, (unsigned int)len2,
+                                srow + rr.front, qrow + rr.front, srow2 + r2.front, qrow2 + r2.front, lane);
+            } else {                                                  /* --include_unmerged: read 1 then read 2, each if it is written */
+                if (fq_written(rr, rr.verdict)) { fq_write_record(d, text, rc, rr, srow, qrow, lane); d += fq_record_size(rc, rr); }
+                if (fq_written(r2, r2.verdict)) fq_write_record(d, M.text2, M.recs2[ri], r2, srow2, qrow2, lane);
+            }
         }
         __syncthreads();
         if (threadIdx.x == FQ_T - 1) s_run = s_sz[FQ_T - 1] + sz;

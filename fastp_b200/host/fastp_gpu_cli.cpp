@@ -26,7 +26,7 @@ static Read* readRecord(std::istream& in) {          /* FastqReader::read src/fa
 
 int main(int argc, char** argv) {
     Options opt;
-    std::string in1, in2, out1, out2, json;
+    std::string in1, in2, out1, out2, mergedOut, json;
     int packSize = 1 << 16, maxLen = 0;
     bool deviceFastq = false, phred64 = false;
     bool dedup = false, evalDup = true; int dupLevel = 0;     /* src/main.cpp:200-209 */
@@ -59,6 +59,8 @@ int main(int argc, char** argv) {
         else if (a == "-y" || a == "--low_complexity_filter") opt.complexityFilter.enabled = true;
         else if (a == "-Y" || a == "--complexity_threshold") opt.complexityFilter.threshold = std::min(100, std::max(0, atoi(next()))) / 100.0;
         else if (a == "-c" || a == "--correction") opt.correction.enabled = true;
+        else if (a == "-m" || a == "--merge") opt.merge.enabled = true; else if (a == "--merged_out") mergedOut = next();
+        else if (a == "--include_unmerged") opt.merge.includeUnmerged = true;
         else if (a == "--overlap_len_require") opt.overlapRequire = atoi(next()); else if (a == "--overlap_diff_limit") opt.overlapDiffLimit = atoi(next());
         else if (a == "--overlap_diff_percent_limit") opt.overlapDiffPercentLimit = atoi(next());
         else if (a == "--device_fastq") deviceFastq = true; else if (a == "-6" || a == "--phred64") phred64 = true;
@@ -69,8 +71,19 @@ int main(int argc, char** argv) {
         else if (a == "--max_read_len") maxLen = atoi(next()); else if (a == "--pack_size") packSize = atoi(next());
         else { fprintf(stderr, "unknown flag %s\n", a.c_str()); return 2; }
     }
-    if (in1.empty()) { fprintf(stderr, "usage: fastp_gpu_cli -i R1.fq [-I R2.fq] [-o out1.fq] [-O out2.fq] [-j summary.json] [fastp flags]\n"); return 2; }
+    if (in1.empty()) { fprintf(stderr, "usage: fastp_gpu_cli -i R1.fq [-I R2.fq] [-o out1.fq] [-O out2.fq] [-m --merged_out merged.fq] [-j summary.json] [fastp flags]\n"); return 2; }
     opt.paired = !in2.empty();
+    if (opt.merge.enabled) {                            /* src/options.cpp:112-147; --stdout and the 0.19.8 rule (--out1 as the merged file) are not taken over */
+        if (!deviceFastq) { fprintf(stderr, "ERROR: merging mode needs --device_fastq\n"); return 2; }
+        if (in2.empty()) { fprintf(stderr, "ERROR: read2 input should be specified by --in2 for merging mode\n"); return 2; }
+        opt.correction.enabled = true;
+        if (opt.merge.includeUnmerged) {
+            if (!out1.empty()) { std::cerr << "You specified --include_unmerged in merging mode. Ignoring argument --out1 = " << out1 << std::endl; out1.clear(); }
+            if (!out2.empty()) { std::cerr << "You specified --include_unmerged in merging mode. Ignoring argument --out2 = " << out2 << std::endl; out2.clear(); }
+        }
+        if (mergedOut.empty()) { fprintf(stderr, "ERROR: In merging mode, you should specify --merged_out\n"); return 2; }
+        if (mergedOut == out1 || mergedOut == out2) { fprintf(stderr, "ERROR: --merged_out and --out1 / --out2 shouldn't have same file name\n"); return 2; }
+    }
     std::ifstream f1(in1), f2;
     if (opt.paired) f2.open(in2);
     if (!f1 || (opt.paired && !f2)) { fprintf(stderr, "cannot open input\n"); return 1; }
@@ -89,9 +102,10 @@ int main(int argc, char** argv) {
     if (chunkBytes == 0) chunkBytes = (size_t)packSize * (size_t)(2 * maxLen + 64);
     GpuChainWorker worker(&opt, maxLen, 0, packSize);
     if (!worker.ok()) { fprintf(stderr, "fastp_gpu_cli: %s\n", worker.error().c_str()); return 1; }
-    std::ofstream o1, o2;
+    std::ofstream o1, o2, om;
     if (!out1.empty()) o1.open(out1);
     if (!out2.empty()) o2.open(out2);
+    if (opt.merge.enabled) om.open(mergedOut);
     if (deviceFastq) {
         if (evalDup || dedup) {                            /* accuracy level: 3 with --dedup, else 1, unless given (src/main.cpp:203-209) */
             if (!worker.setDedup(dupLevel ? dupLevel : (dedup ? 3 : 1), dedup)) { fprintf(stderr, "fastp_gpu_cli: duplicate filter: %s\n", fp_last_error()); return 1; }
@@ -115,7 +129,7 @@ int main(int argc, char** argv) {
             if ((size_t)got < chunkBytes) eof = true;
         };
         auto gz_name = [](const std::string& n) { return n.size() > 3 && n.compare(n.size() - 3, 3, ".gz") == 0; };
-        const bool zout1 = gz_name(out1), zout2 = gz_name(out2);
+        const bool zout1 = gz_name(out1), zout2 = gz_name(out2), zoutm = gz_name(mergedOut);
         std::vector<uint8_t> zbuf;
         auto emit = [&](std::ofstream& o, const std::string& t, bool z) {
             if (!o.is_open() || t.empty()) return;
@@ -131,12 +145,13 @@ int main(int argc, char** argv) {
             fill(g1, buf1, eof1);
             if (opt.paired) fill(g2, buf2, eof2);
             const bool final = eof1 && eof2;
-            std::string s1, s2; size_t c1 = 0, c2 = 0; long units = 0;
-            if (!worker.processFastqText(buf1.data(), buf1.size(), buf2.data(), buf2.size(), final, phred64, &s1, &s2, &c1, &c2, &units)) {
+            std::string s1, s2, sm; size_t c1 = 0, c2 = 0; long units = 0;
+            if (!worker.processFastqText(buf1.data(), buf1.size(), buf2.data(), buf2.size(), final, phred64, &s1, &s2, &c1, &c2, &units, &sm)) {
                 fprintf(stderr, "fastp_gpu_cli: %s\n", worker.error().c_str()); return 1;
             }
             emit(o1, s1, zout1);
             emit(o2, s2, zout2);
+            emit(om, sm, zoutm);
             buf1.erase(0, c1); if (opt.paired) buf2.erase(0, c2);
             if (worker.inputEnded()) break;                    /* a reader gave up on a record: the reference stops reading there */
             if (final && (units == 0 || (buf1.empty() && buf2.empty()))) break;

@@ -45,6 +45,7 @@ struct Options {
     struct { bool enabled = true; std::string sequence, sequenceR2; std::vector<std::string> seqsInFasta;
              bool hasSeqR1 = false, hasSeqR2 = false, hasFasta = false, allowGapOverlapTrimming = false; int dimerMaxLen = 2; } adapter;
     struct { bool enabled = false; } correction;
+    struct { bool enabled = false, includeUnmerged = false; } merge;              /* options.h:104-121 (text path only) */
     struct { bool enabled = true; char qualifiedQual = '0'; int unqualifiedPercentLimit = 40, nBaseLimit = 5, avgQualReq = 0; } qualfilter;
     struct { bool enabled = true; int requiredLength = 15, maxLength = 0; } lengthFilter;
     struct { bool enabled = false; double threshold = 0.3; } complexityFilter;
@@ -93,7 +94,9 @@ public:
 
     /* Text path (device FASTQ codec, SURVEY 8f rank 1): one chunk of plain FASTQ text per side in, the passing reads' text out.
      * Replaces the reader's parse (FastqReader::read), the body above and Read::appendToString in one call; `consumed*` says how many
-     * bytes of each chunk were used -- the caller prepends the rest to its next chunk.  `final`: no more input follows.        */
+     * bytes of each chunk were used -- the caller prepends the rest to its next chunk.  `final`: no more input follows.
+     * With Options::merge.enabled `merged` receives the --merged_out stream (merged reads, and with includeUnmerged the passing reads
+     * of pairs that did not merge; src/peprocessor.cpp:519-560) and outstr1 / outstr2 only the pairs that took neither branch. */
     /* true once a reader rejected a record (strand line not '+', |quality| != |sequence|): like FastqReader::read returning NULL the
      * input ENDS there -- the caller stops feeding chunks (src/fastqreader.cpp:349-364) */
     bool inputEnded() const { return mInputEnded; }
@@ -101,7 +104,8 @@ public:
     bool setDedup(int accuracyLevel, bool dedup) { return mCtx && fp_fastq_set_dedup(mCtx, accuracyLevel, dedup ? 1 : 0) == FP_OK; }
     bool dupTotals(long* total, long* dups) { int64_t t = 0, d = 0; if (!mCtx || fp_dup_totals(mCtx, &t, &d) != FP_OK) return false; *total = (long)t; *dups = (long)d; return true; }
     bool processFastqText(const char* text1, size_t n1, const char* text2, size_t n2, bool final, bool phred64,
-                          std::string* outstr1, std::string* outstr2, size_t* consumed1, size_t* consumed2, long* units);
+                          std::string* outstr1, std::string* outstr2, size_t* consumed1, size_t* consumed2, long* units,
+                          std::string* merged = nullptr);
 
     /* end of run: what Stats::merge / FilterResult::merge hand to the reporters (src/peprocessor.cpp:217-234) */
     bool finish(Stats* pre1, Stats* post1, Stats* pre2, Stats* post2, FilterResult* fr, std::vector<long>* insertSizeHist);
@@ -119,7 +123,7 @@ private:
     uint16_t* mLen[2] = {nullptr, nullptr};
     fp_read_result* mRes[2] = {nullptr, nullptr};
     fp_ov_result* mOv = nullptr;
-    std::vector<uint8_t> mTextOut[2];
+    std::vector<uint8_t> mTextOut[3];      /* out1, out2, merged */
     bool mInputEnded = false;
     std::string mError;
 };

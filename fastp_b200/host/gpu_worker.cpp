@@ -29,7 +29,8 @@ void Options::toParams(fp_params* p, std::vector<const char*>& fastaKeep, std::v
     if (adapter.hasFasta) for (auto& s : adapter.seqsInFasta) fastaKeep.push_back(s.c_str());
     p->n_fasta_adapters = (int)fastaKeep.size(); p->fasta_adapters = fastaKeep.empty() ? nullptr : fastaKeep.data();
     p->allow_gap_overlap_trimming = adapter.allowGapOverlapTrimming; p->dimer_max_len = adapter.dimerMaxLen;
-    p->correction_enabled = correction.enabled;
+    p->correction_enabled = correction.enabled || merge.enabled;           /* options.cpp:120-121 */
+    p->merge_enabled = merge.enabled; p->merge_include_unmerged = merge.includeUnmerged;
     p->overlap_require = overlapRequire; p->overlap_diff_limit = overlapDiffLimit; p->overlap_diff_percent_limit = overlapDiffPercentLimit;
     p->qual_filter_enabled = qualfilter.enabled; p->qualified_qual = (unsigned char)qualfilter.qualifiedQual;
     p->unqualified_percent_limit = qualfilter.unqualifiedPercentLimit; p->n_base_limit = qualfilter.nBaseLimit; p->avg_qual_req = qualfilter.avgQualReq;
@@ -92,7 +93,8 @@ GpuChainWorker::GpuChainWorker(const Options* opt, int maxReadLen, int device, i
     opt->toParams(&mParams, mFastaKeep, mOvr1Keep, mOvr2Keep);
     mStride = std::max(16, (maxReadLen + 15) / 16 * 16);
     mCap = maxBatch;
-    int rc = fp_ctx_create(&mParams, device, maxBatch, mStride, mStride, &mCtx);
+    /* a merged read is up to two rows long: the per-cycle counters need that many cycles */
+    int rc = fp_ctx_create(&mParams, device, maxBatch, mStride, mParams.merge_enabled ? 2 * mStride : mStride, &mCtx);
     if (rc != FP_OK) { mError = fp_last_error(); mCtx = nullptr; return; }
     const int sides = opt->paired ? 2 : 1;
     for (int s = 0; s < sides; s++) {
@@ -172,17 +174,26 @@ bool GpuChainWorker::processPairEnd(ReadPack* leftPack, ReadPack* rightPack, std
 }
 
 bool GpuChainWorker::processFastqText(const char* text1, size_t n1, const char* text2, size_t n2, bool final, bool phred64,
-                                      std::string* outstr1, std::string* outstr2, size_t* consumed1, size_t* consumed2, long* units) {
-    const bool paired = mParams.paired != 0;
-    int64_t ob1 = 0, ob2 = 0, nu = 0, c1 = 0, c2 = 0;
+                                      std::string* outstr1, std::string* outstr2, size_t* consumed1, size_t* consumed2, long* units,
+                                      std::string* merged) {
+    const bool paired = mParams.paired != 0, merging = paired && mParams.merge_enabled;
+    int64_t ob1 = 0, ob2 = 0, obm = 0, nu = 0, c1 = 0, c2 = 0;
     fp_fastq_info i1, i2;
     mTextOut[0].resize(n1 + 64);
     if (paired) mTextOut[1].resize(n2 + 64);
-    const int rc = fp_fastq_process_host(mCtx, reinterpret_cast<const uint8_t*>(text1), (int64_t)n1, paired ? reinterpret_cast<const uint8_t*>(text2) : nullptr,
-                                         paired ? (int64_t)n2 : 0, final ? 1 : 0, phred64 ? 1 : 0,
-                                         mTextOut[0].data(), (int64_t)mTextOut[0].size(), &ob1,
-                                         paired ? mTextOut[1].data() : nullptr, paired ? (int64_t)mTextOut[1].size() : 0, paired ? &ob2 : nullptr,
-                                         &nu, &c1, paired ? &c2 : nullptr, &i1, paired ? &i2 : nullptr);
+    const uint8_t* t1 = reinterpret_cast<const uint8_t*>(text1); const uint8_t* t2 = paired ? reinterpret_cast<const uint8_t*>(text2) : nullptr;
+    int rc;
+    if (merging) {
+        /* everything both inputs hold can land on the merged stream, each merged read with its name suffix (one per pair, i.e. per 8 lines at least) */
+        mTextOut[2].resize(n1 + n2 + (n1 / 8 + 1) * 40 + 64);
+        rc = fp_fastq_process_host_merge(mCtx, t1, (int64_t)n1, t2, (int64_t)n2, final ? 1 : 0, phred64 ? 1 : 0,
+                                         mTextOut[0].data(), (int64_t)mTextOut[0].size(), &ob1, mTextOut[1].data(), (int64_t)mTextOut[1].size(), &ob2,
+                                         mTextOut[2].data(), (int64_t)mTextOut[2].size(), &obm, &nu, &c1, &c2, &i1, &i2);
+    } else
+        rc = fp_fastq_process_host(mCtx, t1, (int64_t)n1, t2, paired ? (int64_t)n2 : 0, final ? 1 : 0, phred64 ? 1 : 0,
+                                   mTextOut[0].data(), (int64_t)mTextOut[0].size(), &ob1,
+                                   paired ? mTextOut[1].data() : nullptr, paired ? (int64_t)mTextOut[1].size() : 0, paired ? &ob2 : nullptr,
+                                   &nu, &c1, paired ? &c2 : nullptr, &i1, paired ? &i2 : nullptr);
     if (rc != FP_OK) { mError = fp_last_error(); return false; }
     if (i1.error == FP_FQ_ERR_STRIDE || (paired && i2.error == FP_FQ_ERR_STRIDE)) { mError = "a read is longer than the row stride (raise --max_read_len)"; return false; }
     if (i1.error != FP_FQ_OK || (paired && i2.error != FP_FQ_OK)) {
@@ -193,6 +204,7 @@ bool GpuChainWorker::processFastqText(const char* text1, size_t n1, const char* 
     }
     if (outstr1) outstr1->append(reinterpret_cast<const char*>(mTextOut[0].data()), (size_t)ob1);
     if (paired && outstr2) outstr2->append(reinterpret_cast<const char*>(mTextOut[1].data()), (size_t)ob2);
+    if (merging && merged) merged->append(reinterpret_cast<const char*>(mTextOut[2].data()), (size_t)obm);
     if (consumed1) *consumed1 = (size_t)c1;
     if (consumed2) *consumed2 = (size_t)c2;
     if (units) *units = (long)nu;

@@ -454,6 +454,40 @@ int  fp_fastq_process_host(fp_ctx* ctx, const uint8_t* text1, int64_t nbytes1, c
                            uint8_t* out2, int64_t out_cap2, int64_t* out_bytes2,
                            int64_t* n_units, int64_t* consumed1, int64_t* consumed2, fp_fastq_info* info1, fp_fastq_info* info2);
 
+/* Merging mode (--merge, fp_params.merge_enabled) writes three streams, decided per pair from its two records (src/peprocessor.cpp:519-622):
+ *   merged pair (FP_F_MERGED): if the merged read passes, ONE record on the merged stream, whatever the duplicate flag says (:528-534) --
+ *       read 1's name line + " merged_<len1>_<len2>", r1[0, len1) + reverse complement of r2[0, len2) (fp_merged_lens; complement as
+ *       src/simd.cpp:296-308: A<->T, C<->G in either case -> upper case, anything else -> 'N'), read 1's strand line (with the same suffix
+ *       unless it is exactly "+"), q1[0, len1) + q2[0, len2) reversed (OverlapAnalysis::merge, src/overlapanalysis.cpp:148-179);
+ *   not merged, --include_unmerged, neither read dropped: read 1 on the merged stream if its own verdict passes and the pair is not a
+ *       flagged duplicate, then read 2 likewise (:537-556);
+ *   every other pair: both reads to their sides under the ordinary rule (pair verdict passes, not a duplicate; :575-584).
+ * fp_fastq_encode_merge writes ONE of the streams of a batch the chain has worked on (fp_process_pe with `ov`), all pointers DEVICE:
+ *   which                FP_FQ_OUT_MERGED (--merged_out), FP_FQ_OUT_R1 (--out1) or FP_FQ_OUT_R2 (--out2)
+ *   d_text1/2, d_recs1/2 the chunks fp_fastq_decode read and the records it wrote, per side (name and strand lines are copied from there)
+ *   d_res1/2, d_ov       what fp_process_pe wrote: records of both reads and the second overlap analysis (:523) of every pair
+ *   d_seq1/2, d_qual1/2  the rows as the chain left them (corrected bases included), ctx stride
+ *   n, d_out, out_cap, out_bytes  as fp_fastq_encode: *out_bytes = size of the whole stream; a record that does not fit under out_cap
+ *                        is left out whole.
+ * FP_E_INVAL on a single-end ctx or one created without merge_enabled.  Synchronous. */
+#define FP_FQ_OUT_MERGED 0
+#define FP_FQ_OUT_R1     1
+#define FP_FQ_OUT_R2     2
+int  fp_fastq_encode_merge(fp_ctx* ctx, int32_t which, const uint8_t* d_text1, const fp_fastq_rec* d_recs1, const uint8_t* d_text2, const fp_fastq_rec* d_recs2,
+                           const fp_read_result* d_res1, const fp_read_result* d_res2, const fp_ov_result* d_ov,
+                           const uint8_t* d_seq1, const uint8_t* d_qual1, const uint8_t* d_seq2, const uint8_t* d_qual2,
+                           int64_t n, uint8_t* d_out, int64_t out_cap, int64_t* out_bytes);
+/* fp_fastq_process_host for a ctx that merges pairs: the same rounds, with the merged stream as a third host output (NULL = not wanted,
+ * like out1 / out2).  With fp_fastq_set_dedup a merged read is written whatever its flag says; the other two cases honour it.
+ * fp_fastq_process_host itself refuses such a ctx (FP_E_INVAL, nothing touched): its two outputs cannot hold what merging writes.
+ * Create the ctx with cycles >= 2 * stride (fp_params.merge_enabled).  FP_E_INVAL on a ctx without merge_enabled. */
+int  fp_fastq_process_host_merge(fp_ctx* ctx, const uint8_t* text1, int64_t nbytes1, const uint8_t* text2, int64_t nbytes2,
+                                 int32_t final_chunk, int32_t phred64,
+                                 uint8_t* out1, int64_t out_cap1, int64_t* out_bytes1,
+                                 uint8_t* out2, int64_t out_cap2, int64_t* out_bytes2,
+                                 uint8_t* merged, int64_t merged_cap, int64_t* merged_bytes,
+                                 int64_t* n_units, int64_t* consumed1, int64_t* consumed2, fp_fastq_info* info1, fp_fastq_info* info2);
+
 /* ---------------- duplication bloom filter (SURVEY.md 8(f) rank 2; src/duplicate.cpp) ----------------
  * fp_dup_check replaces Duplicate::checkRead / checkPair (src/duplicate.cpp:126-154) for a batch in DEVICE memory: d_is_dup[i]
  * (nullable) = what the reference returns for unit i when units are fed in index order, batch after batch -- deterministic, not
@@ -472,7 +506,7 @@ int  fp_dup_reset(fp_ctx* ctx);
  * In merging mode a merged read is counted and written whatever its flag says (src/peprocessor.cpp:528-534); only pairs that did not
  * merge consult it (:547, :553, :575).  The host entry points (fp_process_*_host, _host_packed, _host_patches, fp_fastq_process_host)
  * split their input into chunks and rounds of their own, so one flag array cannot follow them: while a pointer is set they return
- * FP_E_INVAL and touch nothing.  fp_fastq_set_dedup: the text path (fp_fastq_process_host) runs the duplicate filter at
+ * FP_E_INVAL and touch nothing.  fp_fastq_set_dedup: the text path (fp_fastq_process_host, fp_fastq_process_host_merge) runs the duplicate filter at
  * `accuracy_level` on every round's decoded rows before the chain (0 = off) and drops duplicates from the output when `dedup` is set. */
 int  fp_set_dup_flags(fp_ctx* ctx, const uint8_t* d_is_dup);
 int  fp_fastq_set_dedup(fp_ctx* ctx, int32_t accuracy_level, int32_t dedup);
