@@ -114,6 +114,9 @@ class FastqInfo(C.Structure):
 FP_B_INDEXED = 0x1          # fp_batch.flags
 FP_B_PACK2BIT = 0x2
 FP_FQ_OUT_MERGED, FP_FQ_OUT_R1, FP_FQ_OUT_R2 = 0, 1, 2   # fp_fastq_encode_merge `which`
+FP_FQ_OUT_UNPAIRED1, FP_FQ_OUT_UNPAIRED2, FP_FQ_OUT_FAILED = 3, 4, 5   # fp_fastq_encode_rejects `which`
+FP_FQ_OUTS = 6                                           # fp_fastq_process_host_outs: buffers indexed by FP_FQ_OUT_*
+FP_FQ_W_UNPAIRED1, FP_FQ_W_UNPAIRED2 = 0x1, 0x2          # fp_fastq_encode_rejects `writers`
 
 SYMBOLS = {
     "fp_params_default": (None, [C.POINTER(Params), C.c_int]),
@@ -179,6 +182,12 @@ SYMBOLS = {
                                               C.c_void_p, C.c_int64, C.POINTER(C.c_int64),
                                               C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
                                               C.POINTER(FastqInfo), C.POINTER(FastqInfo)]),
+    "fp_fastq_encode_rejects": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32] + [C.c_void_p] * 12 + [C.c_int64, C.c_void_p, C.c_int64,
+                                                                                                   C.POINTER(C.c_int64)]),
+    "fp_fastq_process_host_outs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
+                                             C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                             C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                             C.POINTER(FastqInfo), C.POINTER(FastqInfo)]),
 }
 
 

@@ -109,7 +109,7 @@ struct fp_ctx {
     /* FASTQ codec workspaces (grown on demand) and the buffers of fp_fastq_process_host */
     struct Buf { void* p = nullptr; size_t cap = 0; };
     Buf fq_term, fq_bcnt, fq_agg, fq_bstate, fq_brec, fq_recline, fq_recend, fq_info, fq_bsum;
-    Buf fqh_text[2], fqh_seq[2], fqh_qual[2], fqh_len[2], fqh_recs[2], fqh_res[2], fqh_ov, fqh_out[2], fqh_outbuf[2][3], fqh_recend[2];
+    Buf fqh_text[2], fqh_seq[2], fqh_qual[2], fqh_len[2], fqh_recs[2], fqh_res[2], fqh_ov, fqh_out[2], fqh_outbuf[2][6], fqh_recend[2];
     unsigned int *fq_hinfo = nullptr, *fq_hinfo_dev = nullptr;      /* mapped pinned control words */
     cudaStream_t fq_stream_out = nullptr;
     cudaEvent_t fq_ev_up = nullptr, fq_ev_out[2] = {nullptr, nullptr};
@@ -462,7 +462,8 @@ extern "C" void fp_ctx_destroy(fp_ctx* c) {
         fp_ctx::Buf* all[] = {&c->fq_term, &c->fq_bcnt, &c->fq_agg, &c->fq_bstate, &c->fq_brec, &c->fq_recline, &c->fq_recend, &c->fq_info, &c->fq_bsum,
                               &c->fqh_text[0], &c->fqh_text[1], &c->fqh_seq[0], &c->fqh_seq[1], &c->fqh_qual[0], &c->fqh_qual[1], &c->fqh_len[0], &c->fqh_len[1],
                               &c->fqh_recs[0], &c->fqh_recs[1], &c->fqh_res[0], &c->fqh_res[1], &c->fqh_ov, &c->fqh_out[0], &c->fqh_out[1],
-                              &c->fqh_outbuf[0][0], &c->fqh_outbuf[0][1], &c->fqh_outbuf[0][2], &c->fqh_outbuf[1][0], &c->fqh_outbuf[1][1], &c->fqh_outbuf[1][2], &c->fqh_recend[0], &c->fqh_recend[1], &c->fq_dupflags};
+                              &c->fqh_recend[0], &c->fqh_recend[1], &c->fq_dupflags};
+        for (auto& round : c->fqh_outbuf) for (auto& b : round) fq_free(b);
         if (c->dup.bits) cudaFree(c->dup.bits);
         cudaFree(c->d_dup_primes); cudaFree(c->d_dup_count);
         fq_free(c->dup_pos); fq_free(c->dup_keys); fq_free(c->dup_vals);
@@ -1421,14 +1422,50 @@ extern "C" int fp_fastq_encode_merge(fp_ctx* c, int32_t which, const uint8_t* d_
     return fastq_encode_impl<FQ_SEL_MERGED>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
 }
 
-/* The round loop of the text path.  merging: the ctx merges pairs, so every round also keeps the chain's overlap results and encodes a
-   third stream (outs[2] = --merged_out) beside the two sides. */
+/* the argument rules of fp_fastq_encode_rejects and fp_fastq_process_host_outs (options.cpp:136-143, :222-229) */
+static int fastq_rejects_check(const fp_ctx* c, int writers) {
+    if (writers & ~(FP_FQ_W_UNPAIRED1 | FP_FQ_W_UNPAIRED2)) return set_err(FP_E_INVAL, "writers holds bits other than FP_FQ_W_UNPAIRED1 / FP_FQ_W_UNPAIRED2");
+    if (writers && !c->p.paired) return set_err(FP_E_INVAL, "unpaired outputs need a paired ctx (the reference ignores them for single-end data)");
+    if (writers && c->p.merge_enabled && c->p.merge_include_unmerged)
+        return set_err(FP_E_INVAL, "unpaired outputs with merge_include_unmerged (the reference ignores them: every pair is merged or written whole)");
+    return FP_OK;
+}
+
+extern "C" int fp_fastq_encode_rejects(fp_ctx* c, int32_t which, int32_t writers, const uint8_t* d_text1, const fp_fastq_rec* d_recs1,
+                                       const uint8_t* d_text2, const fp_fastq_rec* d_recs2, const fp_read_result* d_res1, const fp_read_result* d_res2,
+                                       const uint8_t* d_seq1, const uint8_t* d_qual1, const uint16_t* d_len1,
+                                       const uint8_t* d_seq2, const uint8_t* d_qual2, const uint16_t* d_len2,
+                                       int64_t n, uint8_t* d_out, int64_t out_cap, int64_t* out_bytes) {
+    if (!c || !out_bytes) return set_err(FP_E_INVAL, "null argument");
+    *out_bytes = 0;
+    if (which != FP_FQ_OUT_UNPAIRED1 && which != FP_FQ_OUT_UNPAIRED2 && which != FP_FQ_OUT_FAILED)
+        return set_err(FP_E_INVAL, "which must be FP_FQ_OUT_UNPAIRED1, FP_FQ_OUT_UNPAIRED2 or FP_FQ_OUT_FAILED");
+    if (which != FP_FQ_OUT_FAILED && !c->p.paired) return set_err(FP_E_INVAL, "unpaired outputs need a paired ctx (the reference ignores them for single-end data)");
+    int rc;
+    if ((rc = fastq_rejects_check(c, writers))) return rc;
+    if (n <= 0) return FP_OK;
+    const bool pe = c->p.paired != 0;
+    if (!d_text1 || !d_recs1 || !d_res1 || !d_seq1 || !d_qual1 || !d_len1 || (out_cap > 0 && !d_out) ||
+        (pe && (!d_text2 || !d_recs2 || !d_res2 || !d_seq2 || !d_qual2 || !d_len2)))
+        return set_err(FP_E_INVAL, "null argument");
+    fq_merge_args M{};
+    M.len1 = d_len1; M.writers = writers; M.merging = pe && c->p.merge_enabled; M.include_unmerged = c->p.merge_include_unmerged ? 1 : 0;
+    if (pe) { M.text2 = d_text2; M.recs2 = reinterpret_cast<const fq_rec*>(d_recs2); M.res2 = d_res2; M.seq2 = d_seq2; M.qual2 = d_qual2; M.len2 = d_len2; }
+    if (which == FP_FQ_OUT_UNPAIRED1) return fastq_encode_impl<FQ_SEL_UNPAIRED1>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
+    if (which == FP_FQ_OUT_UNPAIRED2) return fastq_encode_impl<FQ_SEL_UNPAIRED2>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
+    return fastq_encode_impl<FQ_SEL_FAILED>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
+}
+
+/* The round loop of the text path.  outs / ocap / out_bytes are indexed by FP_FQ_OUT_*; a NULL buffer is not encoded.  merging: the ctx
+   merges pairs, so every round also keeps the chain's overlap results for the merged stream.  The reject streams read the round's decoded
+   lengths (fqh_len, which the chain leaves as they are) and take the unpaired writers from which unpaired buffers are given. */
 static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbytes1, const uint8_t* text2, int64_t nbytes2,
-                                   int32_t final_chunk, int32_t phred64, uint8_t* const outs[3], const int64_t ocap[3], int64_t* const out_bytes[3],
+                                   int32_t final_chunk, int32_t phred64, uint8_t* const outs[FP_FQ_OUTS], const int64_t ocap[FP_FQ_OUTS],
+                                   int64_t* const out_bytes[FP_FQ_OUTS],
                                    int64_t* n_units, int64_t* consumed1, int64_t* consumed2, fp_fastq_info* info1, fp_fastq_info* info2) {
     const int sides = c->p.paired ? 2 : 1;
     const bool merging = c->p.merge_enabled && sides == 2;
-    const int nstreams = merging ? 3 : sides;
+    const int writers = (outs[FP_FQ_OUT_UNPAIRED1] ? FP_FQ_W_UNPAIRED1 : 0) | (outs[FP_FQ_OUT_UNPAIRED2] ? FP_FQ_W_UNPAIRED2 : 0);
     if (c->dup_flags) return set_err(FP_E_INVAL, "duplicate flags are set (fp_set_dup_flags): the text path runs its own duplicate filter (fp_fastq_set_dedup)");
     CK(cudaSetDevice(c->device));
     cudaStream_t st = c->stream[0], up = c->stream[1];
@@ -1456,7 +1493,7 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
         if ((rc = fq_ensure(c->fqh_res[s], (size_t)cap * sizeof(fp_read_result)))) return rc;
     }
     if (merging && (rc = fq_ensure(c->fqh_ov, (size_t)cap * sizeof(fp_ov_result)))) return rc;
-    int64_t upl[2] = {0, 0}, start[2] = {0, 0}, obytes[3] = {0, 0, 0}, units = 0;
+    int64_t upl[2] = {0, 0}, start[2] = {0, 0}, obytes[FP_FQ_OUTS] = {0}, units = 0;
     fp_fastq_info agg[2]; memset(agg, 0, sizeof(agg)); agg[0].error_record = agg[1].error_record = -1;
     int flip = 0;
     auto upload_more = [&]() -> int {
@@ -1525,24 +1562,32 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
             if (rc) return rc;
             CK(cudaEventSynchronize(c->fq_ev_out[flip]));        /* the output buffers of two rounds ago have gone down */
             const uint8_t* rtext[2] = {(const uint8_t*)c->fqh_text[0].p + rstart[0], sides == 2 ? (const uint8_t*)c->fqh_text[1].p + rstart[1] : nullptr};
-            for (int s = 0; s < nstreams; s++) {
+            for (int s = 0; s < FP_FQ_OUTS; s++) {
                 if (!outs[s]) continue;                           /* caller does not want this stream's text */
                 fp_ctx::Buf& ob = c->fqh_outbuf[flip][s];
                 const int64_t room = std::max<int64_t>(ocap[s] - obytes[s], 0);
-                /* per unit: one record of a side; on the merged stream one read of up to two rows, or two records */
-                int64_t want = std::min<int64_t>(room, n * (int64_t)(s == 2 ? 4 * c->stride + 512 : 2 * c->stride + 256));
+                /* per unit: one record of a side; on the merged stream one read of up to two rows, or two records; on the failed stream two
+                   tagged records */
+                const bool two = s == FP_FQ_OUT_MERGED || s == FP_FQ_OUT_FAILED;
+                int64_t want = std::min<int64_t>(room, n * (int64_t)(two ? 4 * c->stride + 512 : 2 * c->stride + 256));
                 int64_t total = 0;
+                const fp_fastq_rec* recs[2] = {(const fp_fastq_rec*)c->fqh_recs[0].p, (const fp_fastq_rec*)c->fqh_recs[1].p};
+                const fp_read_result* res[2] = {(const fp_read_result*)c->fqh_res[0].p, (const fp_read_result*)c->fqh_res[1].p};
+                const uint8_t* seq[2] = {(const uint8_t*)c->fqh_seq[0].p, (const uint8_t*)c->fqh_seq[1].p};
+                const uint8_t* qual[2] = {(const uint8_t*)c->fqh_qual[0].p, (const uint8_t*)c->fqh_qual[1].p};
                 for (int attempt = 0; attempt < 2; attempt++) {   /* names longer than the estimate: encode again into a buffer of the exact size */
                     if ((rc = fq_ensure(ob, (size_t)want + 64))) return rc;
-                    if (merging)
-                        rc = fp_fastq_encode_merge(c, s == 2 ? FP_FQ_OUT_MERGED : s == 0 ? FP_FQ_OUT_R1 : FP_FQ_OUT_R2,
-                                                   rtext[0], (const fp_fastq_rec*)c->fqh_recs[0].p, rtext[1], (const fp_fastq_rec*)c->fqh_recs[1].p,
-                                                   (const fp_read_result*)c->fqh_res[0].p, (const fp_read_result*)c->fqh_res[1].p, (const fp_ov_result*)c->fqh_ov.p,
-                                                   (const uint8_t*)c->fqh_seq[0].p, (const uint8_t*)c->fqh_qual[0].p, (const uint8_t*)c->fqh_seq[1].p,
-                                                   (const uint8_t*)c->fqh_qual[1].p, n, (uint8_t*)ob.p, want, &total);
-                    else
-                        rc = fp_fastq_encode(c, rtext[s], (const fp_fastq_rec*)c->fqh_recs[s].p, (const fp_read_result*)c->fqh_res[s].p,
-                                             (const uint8_t*)c->fqh_seq[s].p, (const uint8_t*)c->fqh_qual[s].p, n, (uint8_t*)ob.p, want, &total);
+                    if (s >= FP_FQ_OUT_UNPAIRED1)
+                        rc = fp_fastq_encode_rejects(c, s, writers, rtext[0], recs[0], rtext[1], recs[1], res[0], res[1], seq[0], qual[0],
+                                                     (const uint16_t*)c->fqh_len[0].p, seq[1], qual[1], (const uint16_t*)c->fqh_len[1].p,
+                                                     n, (uint8_t*)ob.p, want, &total);
+                    else if (merging)
+                        rc = fp_fastq_encode_merge(c, s, rtext[0], recs[0], rtext[1], recs[1], res[0], res[1], (const fp_ov_result*)c->fqh_ov.p,
+                                                   seq[0], qual[0], seq[1], qual[1], n, (uint8_t*)ob.p, want, &total);
+                    else {
+                        const int side = s == FP_FQ_OUT_R2 ? 1 : 0;
+                        rc = fp_fastq_encode(c, rtext[side], recs[side], res[side], seq[side], qual[side], n, (uint8_t*)ob.p, want, &total);
+                    }
                     if (rc) return rc;
                     if (total <= want) break;
                     if (total > room) return set_err(FP_E_TOOLARGE, "output buffer too small for the encoded FASTQ text");
@@ -1566,7 +1611,7 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
     if (trace) fprintf(stderr, "[fq] loop %.2f ms, drain %.2f ms\n", t_loop - t_begin, now() - t_loop);
     agg[0].consumed = start[0]; agg[1].consumed = start[1];
     *n_units = units; *consumed1 = start[0]; if (consumed2) *consumed2 = start[1];
-    for (int s = 0; s < 3; s++) if (out_bytes[s]) *out_bytes[s] = obytes[s];
+    for (int s = 0; s < FP_FQ_OUTS; s++) if (out_bytes[s]) *out_bytes[s] = obytes[s];
     if (info1) *info1 = agg[0];
     if (info2 && sides == 2) *info2 = agg[1];
     return FP_OK;
@@ -1580,8 +1625,9 @@ extern "C" int fp_fastq_process_host(fp_ctx* c, const uint8_t* text1, int64_t nb
     if (!c || !n_units || !consumed1 || !out_bytes1) return set_err(FP_E_INVAL, "null argument");
     if (c->p.paired && (!consumed2 || !out_bytes2)) return set_err(FP_E_INVAL, "paired ctx needs the second side");
     if (c->p.paired && c->p.merge_enabled) return set_err(FP_E_INVAL, "ctx merges pairs: use fp_fastq_process_host_merge, which also returns the merged reads");
-    uint8_t* const outs[3] = {out1, out2, nullptr}; const int64_t ocap[3] = {out_cap1, out_cap2, 0};
-    int64_t* const ob[3] = {out_bytes1, out_bytes2, nullptr};
+    uint8_t* const outs[FP_FQ_OUTS] = {nullptr, out1, c->p.paired ? out2 : nullptr, nullptr, nullptr, nullptr};
+    const int64_t ocap[FP_FQ_OUTS] = {0, out_cap1, out_cap2, 0, 0, 0};
+    int64_t* const ob[FP_FQ_OUTS] = {nullptr, out_bytes1, out_bytes2, nullptr, nullptr, nullptr};
     return fastq_process_host_impl(c, text1, nbytes1, text2, nbytes2, final_chunk, phred64, outs, ocap, ob, n_units, consumed1, consumed2, info1, info2);
 }
 
@@ -1594,9 +1640,26 @@ extern "C" int fp_fastq_process_host_merge(fp_ctx* c, const uint8_t* text1, int6
     if (!c || !n_units || !consumed1 || !consumed2 || !out_bytes1 || !out_bytes2 || !merged_bytes) return set_err(FP_E_INVAL, "null argument");
     if (!c->p.paired) return set_err(FP_E_INVAL, "ctx was created for single-end data: merging needs pairs");
     if (!c->p.merge_enabled) return set_err(FP_E_INVAL, "ctx was created without merge_enabled: use fp_fastq_process_host");
-    uint8_t* const outs[3] = {out1, out2, merged}; const int64_t ocap[3] = {out_cap1, out_cap2, merged_cap};
-    int64_t* const ob[3] = {out_bytes1, out_bytes2, merged_bytes};
+    uint8_t* const outs[FP_FQ_OUTS] = {merged, out1, out2, nullptr, nullptr, nullptr};
+    const int64_t ocap[FP_FQ_OUTS] = {merged_cap, out_cap1, out_cap2, 0, 0, 0};
+    int64_t* const ob[FP_FQ_OUTS] = {merged_bytes, out_bytes1, out_bytes2, nullptr, nullptr, nullptr};
     return fastq_process_host_impl(c, text1, nbytes1, text2, nbytes2, final_chunk, phred64, outs, ocap, ob, n_units, consumed1, consumed2, info1, info2);
+}
+
+extern "C" int fp_fastq_process_host_outs(fp_ctx* c, const uint8_t* text1, int64_t nbytes1, const uint8_t* text2, int64_t nbytes2,
+                                          int32_t final_chunk, int32_t phred64, uint8_t* const outs[FP_FQ_OUTS], const int64_t out_caps[FP_FQ_OUTS],
+                                          int64_t out_bytes[FP_FQ_OUTS], int64_t* n_units, int64_t* consumed1, int64_t* consumed2,
+                                          fp_fastq_info* info1, fp_fastq_info* info2) {
+    if (!c || !outs || !out_caps || !out_bytes || !n_units || !consumed1) return set_err(FP_E_INVAL, "null argument");
+    if (c->p.paired && !consumed2) return set_err(FP_E_INVAL, "paired ctx needs the second side");
+    if (!c->p.paired && outs[FP_FQ_OUT_R2]) return set_err(FP_E_INVAL, "an out2 buffer on a single-end ctx");
+    if (outs[FP_FQ_OUT_MERGED] && !(c->p.paired && c->p.merge_enabled)) return set_err(FP_E_INVAL, "a merged buffer on a ctx that does not merge pairs");
+    const int writers = (outs[FP_FQ_OUT_UNPAIRED1] ? FP_FQ_W_UNPAIRED1 : 0) | (outs[FP_FQ_OUT_UNPAIRED2] ? FP_FQ_W_UNPAIRED2 : 0);
+    int rc;
+    if ((rc = fastq_rejects_check(c, writers))) return rc;
+    int64_t* ob[FP_FQ_OUTS];
+    for (int s = 0; s < FP_FQ_OUTS; s++) ob[s] = &out_bytes[s];
+    return fastq_process_host_impl(c, text1, nbytes1, text2, nbytes2, final_chunk, phred64, outs, out_caps, ob, n_units, consumed1, consumed2, info1, info2);
 }
 
 /* ---------------- duplication bloom filter (fp_dup.h / fp_dup.cuh) ---------------- */

@@ -306,21 +306,32 @@ __global__ void fq_set_u32_kernel(unsigned int* p, unsigned int v) { if (!blockI
 __global__ void fq_copy_u32_kernel(const unsigned int* src, unsigned int* dst) { if (!blockIdx.x && !threadIdx.x) *dst = *src; }
 
 /* ---- encode ----
- * One size pass, one scan and one write pass serve four output streams, chosen at compile time:
+ * One size pass, one scan and one write pass serve the output streams, chosen at compile time:
  *   FQ_SEL_PLAIN   every unit whose pair verdict passes and that --dedup did not flag (peprocessor.cpp:575-584, seprocessor.cpp:268)
  *   FQ_SEL_MERGED  --merged_out: the merged read of a merged pair (peprocessor.cpp:528-534; the duplicate flag is not consulted),
  *                  or with --include_unmerged read 1 then read 2 of a pair that did not merge, each by its own verdict (:537-556)
  *   FQ_SEL_SIDE    --out1 / --out2 in merging mode: only units that took neither merging branch (:563-585)
- * The primary arrays (text, recs, res, seq, qual) are read 1's for FQ_SEL_MERGED and the written side's for FQ_SEL_SIDE;
- * fq_merge_args carries the other side (FQ_SEL_SIDE reads only its records). */
+ *   FQ_SEL_UNPAIRED1 / FQ_SEL_UNPAIRED2 / FQ_SEL_FAILED
+ *                  --unpaired1 / --unpaired2 / --failed_out: what a unit that is not a flagged duplicate, and that took neither merging
+ *                  branch, writes when exactly one read passes (peprocessor.cpp:594-620), or SE when the read fails (seprocessor.cpp:287-289);
+ *                  see fq_reject_plan
+ * The primary arrays (text, recs, res, seq, qual) are read 1's for FQ_SEL_MERGED and the reject streams, and the written side's for
+ * FQ_SEL_SIDE; fq_merge_args carries the other side (FQ_SEL_SIDE reads only its records). */
 #define FQ_SCAN_ITEMS 2048
 #define FQ_SEL_PLAIN 0
 #define FQ_SEL_MERGED 1
 #define FQ_SEL_SIDE 2
+#define FQ_SEL_UNPAIRED1 3
+#define FQ_SEL_UNPAIRED2 4
+#define FQ_SEL_FAILED 5
 struct fq_merge_args {
     const uint8_t* text2; const fq_rec* recs2; const fp_read_result* res2; const uint8_t* seq2; const uint8_t* qual2;
     const fp_ov_result* ov;
     int include_unmerged;
+    /* reject streams only: decoded lengths of both sides (a dropped read is written whole), which unpaired writers exist
+       (bit 0: --unpaired1, bit 1: a separate --unpaired2), whether the ctx merges; res2 == NULL for single-end */
+    const uint16_t* len1; const uint16_t* len2;
+    int writers, merging;
 };
 /* which branch of peprocessor.cpp:519-622 a unit took, from its two records */
 #define FQ_U_ORDINARY 0
@@ -354,9 +365,111 @@ __device__ __forceinline__ void fq_merged_lens(const fp_ov_result& ov, int r2_le
     len2 = ov.offset > 0 ? r2_len - ov.overlap_len : 0;
 }
 __device__ __forceinline__ bool fq_strand_is_plus(const uint8_t* text, const fq_rec& rc) { return rc.strand_len == 1 && text[rc.strand_off] == '+'; }
+
+/* ---- reject streams (--unpaired1 / --unpaired2 / --failed_out) ----
+ * Tags are FAILED_TYPES (common.h:56-65) indexed by the verdict, plus FQ_TAG_PAIRED for the passing read of a pair whose mate failed.
+ * A tagged record is Read::appendToStringWithTag (read.cpp:136-154): name line, ' ', tag, then the record as appendToString writes it.
+ * The reference writes or1 / or2, the reads as trimAndCut left them in place: the kept window [front, front+len) of the row (corrected
+ * bases included), or for a read trimAndCut dropped (never trimmed or corrected) the whole row [0, decoded length). */
+#define FQ_TAG_PAIRED 32u
+#define FQ_TAG_NONE 0xFFu
+#define FQ_TAG_MAX 24
+__constant__ char fq_tag_text[FQ_TAG_PAIRED + 1][FQ_TAG_MAX] = {
+    "passed", "", "", "", "failed_polyx_filter", "", "", "", "failed_bad_overlap", "", "", "",
+    "failed_too_many_n_bases", "", "", "", "failed_too_short", "failed_too_long", "", "", "failed_quality_filter", "", "", "",
+    "failed_low_complexity", "", "", "", "failed_adapter_dimer", "", "", "", "paired_read_is_failing"};
+__constant__ unsigned char fq_tag_len[FQ_TAG_PAIRED + 1] = {6, 0, 0, 0, 19, 0, 0, 0, 18, 0, 0, 0, 23, 0, 0, 0, 16, 15, 0, 0, 21, 0, 0, 0,
+                                                             21, 0, 0, 0, 20, 0, 0, 0, 22};
+/* The records one unit puts on one reject stream, in writing order, packed in a word: the count (0..2) in bits 0-1, then 9 bits per
+ * record, its side (0 / 1) in the low bit and its tag (FQ_TAG_NONE = untagged) above. */
+__device__ __forceinline__ unsigned int fq_plan1(unsigned int side, unsigned int tag) { return 1u | (side | tag << 1) << 2; }
+__device__ __forceinline__ unsigned int fq_plan2(unsigned int s0, unsigned int t0, unsigned int s1, unsigned int t1) {
+    return 2u | (s0 | t0 << 1) << 2 | (s1 | t1 << 1) << 11;
+}
+__device__ __forceinline__ unsigned int fq_plan_side(unsigned int P, int k) { return (P >> (2 + 9 * k)) & 1u; }
+__device__ __forceinline__ unsigned int fq_plan_tag(unsigned int P, int k) { return (P >> (3 + 9 * k)) & 0xFFu; }
+__device__ __forceinline__ bool fq_passes(const fp_read_result& r) { return !(r.flags & FP_F_DROPPED) && r.verdict == FP_PASS_FILTER; }
+template <int SEL>
+__device__ __forceinline__ unsigned int fq_reject_plan(const fp_read_result& a, const fq_merge_args& M, long long i) {
+    if (a.flags & FP_F_DUPLICATE) return 0u;                                             /* dedupOut (seprocessor.cpp:280, peprocessor.cpp:575) */
+    if (!M.res2) return SEL == FQ_SEL_FAILED && !fq_passes(a) ? fq_plan1(0, a.verdict) : 0u;        /* SE: seprocessor.cpp:281-289 */
+    const fp_read_result& b = M.res2[i];
+    if (M.merging && fq_unit_class(a, b, M.include_unmerged) != FQ_U_ORDINARY) return 0u; /* only the !mergeProcessed branch (:562) */
+    const bool p1 = fq_passes(a), p2 = fq_passes(b);
+    if (p1 == p2) return 0u;                                                             /* both written to out1/out2, or neither anywhere */
+    const bool u1 = M.writers & 1, u2 = M.writers & 2;
+    if (p1) {                                                                            /* :594-603 */
+        if (SEL == FQ_SEL_UNPAIRED1) return u1 ? fq_plan1(0, FQ_TAG_NONE) : 0u;
+        if (SEL == FQ_SEL_FAILED) return u1 ? fq_plan1(1, b.verdict) : fq_plan2(0, FQ_TAG_PAIRED, 1, b.verdict);
+        return 0u;
+    }
+    if (SEL == FQ_SEL_UNPAIRED2) return u2 ? fq_plan1(1, FQ_TAG_NONE) : 0u;              /* :604-619 */
+    if (SEL == FQ_SEL_UNPAIRED1) return u1 && !u2 ? fq_plan1(1, FQ_TAG_NONE) : 0u;
+    return u1 || u2 ? fq_plan1(0, a.verdict) : fq_plan2(0, a.verdict, 1, FQ_TAG_PAIRED);
+}
+/* the row window a reject record writes: [from, from + n) */
+__device__ __forceinline__ void fq_reject_window(const fp_read_result& r, unsigned int decoded_len, unsigned int& from, unsigned int& n) {
+    if (r.flags & FP_F_DROPPED) { from = 0; n = decoded_len; } else { from = r.front; n = r.len; }
+}
+__device__ __forceinline__ unsigned long long fq_tagged_size(const fq_rec& rc, unsigned int tag, unsigned int n) {
+    return (unsigned long long)(rc.name_len & 0x0FFFFFFFu) + (tag == FQ_TAG_NONE ? 0u : 1u + fq_tag_len[tag]) + rc.strand_len + 2ull * n + 4ull;
+}
+/* size of the record of side `side` of unit i with tag `tag` */
+__device__ __forceinline__ unsigned long long fq_reject_record_size(const fq_rec* recs, const fp_read_result* res, const fq_merge_args& M,
+                                                                    unsigned int side, unsigned int tag, long long i) {
+    unsigned int from, n;
+    fq_reject_window(side ? M.res2[i] : res[i], side ? M.len2[i] : M.len1[i], from, n);
+    return fq_tagged_size(side ? M.recs2[i] : recs[i], tag, n);
+}
+template <int SEL>
+__device__ __forceinline__ unsigned long long fq_reject_size(const fq_rec* recs, const fp_read_result* res, const fq_merge_args& M, long long i) {
+    const unsigned int P = fq_reject_plan<SEL>(res[i], M, i);
+    if (SEL != FQ_SEL_FAILED)                                   /* at most one untagged record, of a read that passes: its kept window */
+        return P == 0u ? 0ull : fq_plan_side(P, 0) ? fq_record_size(M.recs2[i], M.res2[i]) : fq_record_size(recs[i], res[i]);
+    unsigned long long s = 0;
+    if ((P & 3u) > 0) s += fq_reject_record_size(recs, res, M, fq_plan_side(P, 0), fq_plan_tag(P, 0), i);
+    if ((P & 3u) > 1) s += fq_reject_record_size(recs, res, M, fq_plan_side(P, 1), fq_plan_tag(P, 1), i);
+    return s;
+}
+/* Read::appendToStringWithTag by one warp (untagged with FQ_TAG_NONE): returns the bytes written */
+__device__ __forceinline__ unsigned long long fq_write_tagged(uint8_t* d, const uint8_t* text, const fq_rec& rc, unsigned int tag,
+                                                              const uint8_t* srow, const uint8_t* qrow, unsigned int n, int lane) {
+    uint8_t* const d0 = d;
+    const unsigned int nl = rc.name_len & 0x0FFFFFFFu;
+    for (unsigned int t = lane; t < nl; t += 32) d[t] = text[rc.name_off + t];
+    d += nl;
+    if (tag != FQ_TAG_NONE) {
+        const unsigned int tl = fq_tag_len[tag];
+        if (lane == 0) d[0] = ' ';
+        for (unsigned int t = lane; t < tl; t += 32) d[1 + t] = (uint8_t)fq_tag_text[tag][t];
+        d += 1 + tl;
+    }
+    if (lane == 0) d[0] = '\n';
+    d += 1;
+    for (unsigned int t = lane; t < n; t += 32) d[t] = srow[t];
+    if (lane == 0) d[n] = '\n';
+    d += n + 1;
+    for (unsigned int t = lane; t < rc.strand_len; t += 32) d[t] = text[rc.strand_off + t];
+    if (lane == 0) d[rc.strand_len] = '\n';
+    d += rc.strand_len + 1;
+    for (unsigned int t = lane; t < n; t += 32) d[t] = qrow[t];
+    if (lane == 0) d[n] = '\n';
+    return (unsigned long long)(d + n + 1 - d0);
+}
+/* the record of side `side` of unit i on a reject stream */
+__device__ __forceinline__ unsigned long long fq_write_reject(uint8_t* d, const uint8_t* text, const fq_rec* recs, const fp_read_result* res,
+                                                              const uint8_t* seq, const uint8_t* qual, const fq_merge_args& M,
+                                                              unsigned int side, unsigned int tag, int stride, long long i, int lane) {
+    unsigned int from, n;
+    fq_reject_window(side ? M.res2[i] : res[i], side ? M.len2[i] : M.len1[i], from, n);
+    const size_t row = (size_t)i * stride + from;
+    return fq_write_tagged(d, side ? M.text2 : text, side ? M.recs2[i] : recs[i], tag, (side ? M.seq2 : seq) + row, (side ? M.qual2 : qual) + row, n, lane);
+}
+
 /* bytes unit i puts on the selected stream */
 template <int SEL>
 __device__ __forceinline__ unsigned long long fq_unit_size(const uint8_t* text, const fq_rec* recs, const fp_read_result* res, const fq_merge_args& M, long long i) {
+    if (SEL >= FQ_SEL_UNPAIRED1) return fq_reject_size<SEL>(recs, res, M, i);
     const fp_read_result r = res[i];
     if (SEL == FQ_SEL_PLAIN) return fq_written(r, r.pair_verdict) ? fq_record_size(recs[i], r) : 0ull;
     const fp_read_result r2 = M.res2[i];
@@ -470,6 +583,12 @@ __global__ void __launch_bounds__(FQ_T) fq_encode_kernel(const uint8_t* text, co
             const unsigned long long o = s_sz[j];
             if (need == 0 || o + need > out_cap) continue;            /* a unit that does not fit is skipped whole: caller sees total > cap */
             uint8_t* d = out + o;
+            if (SEL >= FQ_SEL_UNPAIRED1) {                             /* reject streams: the unit's records in plan order */
+                const unsigned int P = fq_reject_plan<SEL>(res[ri], M, ri);
+                d += fq_write_reject(d, text, recs, res, seq, qual, M, fq_plan_side(P, 0), fq_plan_tag(P, 0), stride, ri, lane);
+                if (SEL == FQ_SEL_FAILED && (P & 3u) > 1) fq_write_reject(d, text, recs, res, seq, qual, M, fq_plan_side(P, 1), fq_plan_tag(P, 1), stride, ri, lane);
+                continue;
+            }
             const fp_read_result rr = res[ri];
             const fq_rec rc = recs[ri];
             const uint8_t* srow = seq + (size_t)ri * stride;

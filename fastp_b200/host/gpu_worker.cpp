@@ -175,25 +175,26 @@ bool GpuChainWorker::processPairEnd(ReadPack* leftPack, ReadPack* rightPack, std
 
 bool GpuChainWorker::processFastqText(const char* text1, size_t n1, const char* text2, size_t n2, bool final, bool phred64,
                                       std::string* outstr1, std::string* outstr2, size_t* consumed1, size_t* consumed2, long* units,
-                                      std::string* merged) {
+                                      std::string* merged, std::string* unpaired1, std::string* unpaired2, std::string* failed) {
     const bool paired = mParams.paired != 0, merging = paired && mParams.merge_enabled;
-    int64_t ob1 = 0, ob2 = 0, obm = 0, nu = 0, c1 = 0, c2 = 0;
+    int64_t nu = 0, c1 = 0, c2 = 0;
     fp_fastq_info i1, i2;
-    mTextOut[0].resize(n1 + 64);
-    if (paired) mTextOut[1].resize(n2 + 64);
     const uint8_t* t1 = reinterpret_cast<const uint8_t*>(text1); const uint8_t* t2 = paired ? reinterpret_cast<const uint8_t*>(text2) : nullptr;
-    int rc;
-    if (merging) {
-        /* everything both inputs hold can land on the merged stream, each merged read with its name suffix (one per pair, i.e. per 8 lines at least) */
-        mTextOut[2].resize(n1 + n2 + (n1 / 8 + 1) * 40 + 64);
-        rc = fp_fastq_process_host_merge(mCtx, t1, (int64_t)n1, t2, (int64_t)n2, final ? 1 : 0, phred64 ? 1 : 0,
-                                         mTextOut[0].data(), (int64_t)mTextOut[0].size(), &ob1, mTextOut[1].data(), (int64_t)mTextOut[1].size(), &ob2,
-                                         mTextOut[2].data(), (int64_t)mTextOut[2].size(), &obm, &nu, &c1, &c2, &i1, &i2);
-    } else
-        rc = fp_fastq_process_host(mCtx, t1, (int64_t)n1, t2, paired ? (int64_t)n2 : 0, final ? 1 : 0, phred64 ? 1 : 0,
-                                   mTextOut[0].data(), (int64_t)mTextOut[0].size(), &ob1,
-                                   paired ? mTextOut[1].data() : nullptr, paired ? (int64_t)mTextOut[1].size() : 0, paired ? &ob2 : nullptr,
-                                   &nu, &c1, paired ? &c2 : nullptr, &i1, paired ? &i2 : nullptr);
+    const size_t both = n1 + (paired ? n2 : 0);
+    /* what each stream can hold at most: a side's reads; on the merged stream everything both inputs hold, each merged read with its name
+       suffix (one per pair, i.e. per 8 lines at least); on unpaired1 reads of either side; on the failed stream reads of either side, each
+       with a tag of up to 24 bytes (a record takes 6 bytes at least) */
+    std::string* want[FP_FQ_OUTS] = {merging ? merged : nullptr, outstr1, paired ? outstr2 : nullptr, paired ? unpaired1 : nullptr,
+                                     paired ? unpaired2 : nullptr, failed};
+    const size_t cap[FP_FQ_OUTS] = {n1 + n2 + (n1 / 8 + 1) * 40 + 64, n1 + 64, n2 + 64, both + 64, n2 + 64, both + (both / 6 + 2) * 24 + 64};
+    uint8_t* outs[FP_FQ_OUTS]; int64_t caps[FP_FQ_OUTS], ob[FP_FQ_OUTS];
+    for (int s = 0; s < FP_FQ_OUTS; s++) {
+        if (want[s]) mTextOut[s].resize(cap[s]);
+        outs[s] = want[s] ? mTextOut[s].data() : nullptr;
+        caps[s] = want[s] ? (int64_t)cap[s] : 0;
+    }
+    const int rc = fp_fastq_process_host_outs(mCtx, t1, (int64_t)n1, t2, paired ? (int64_t)n2 : 0, final ? 1 : 0, phred64 ? 1 : 0, outs, caps, ob,
+                                              &nu, &c1, paired ? &c2 : nullptr, &i1, paired ? &i2 : nullptr);
     if (rc != FP_OK) { mError = fp_last_error(); return false; }
     if (i1.error == FP_FQ_ERR_STRIDE || (paired && i2.error == FP_FQ_ERR_STRIDE)) { mError = "a read is longer than the row stride (raise --max_read_len)"; return false; }
     if (i1.error != FP_FQ_OK || (paired && i2.error != FP_FQ_OK)) {
@@ -202,9 +203,8 @@ bool GpuChainWorker::processFastqText(const char* text1, size_t n1, const char* 
                 bad.error == FP_FQ_ERR_STRAND ? "Expected '+'" : "ERROR: sequence and quality have different length:", (long long)bad.error_record, i1.error != FP_FQ_OK ? 1 : 2);
         mInputEnded = true;
     }
-    if (outstr1) outstr1->append(reinterpret_cast<const char*>(mTextOut[0].data()), (size_t)ob1);
-    if (paired && outstr2) outstr2->append(reinterpret_cast<const char*>(mTextOut[1].data()), (size_t)ob2);
-    if (merging && merged) merged->append(reinterpret_cast<const char*>(mTextOut[2].data()), (size_t)obm);
+    for (int s = 0; s < FP_FQ_OUTS; s++)
+        if (want[s]) want[s]->append(reinterpret_cast<const char*>(mTextOut[s].data()), (size_t)ob[s]);
     if (consumed1) *consumed1 = (size_t)c1;
     if (consumed2) *consumed2 = (size_t)c2;
     if (units) *units = (long)nu;

@@ -488,6 +488,53 @@ int  fp_fastq_process_host_merge(fp_ctx* ctx, const uint8_t* text1, int64_t nbyt
                                  uint8_t* merged, int64_t merged_cap, int64_t* merged_bytes,
                                  int64_t* n_units, int64_t* consumed1, int64_t* consumed2, fp_fastq_info* info1, fp_fastq_info* info2);
 
+/* Reads that do not go to out1 / out2: --unpaired1, --unpaired2 and --failed_out (src/seprocessor.cpp:280-290, src/peprocessor.cpp:575-620).
+ * Only a unit that is not a flagged duplicate and, in merging mode, took neither merging branch (not merged, not covered by
+ * --include_unmerged) writes here.  A read "passes" when trimAndCut kept it and its own verdict (after the adapter-dimer override) is
+ * FP_PASS_FILTER.  Single-end: a read that does not pass goes to failed, tagged with its reason.  Paired-end, by the writers that exist:
+ *   both pass, or neither (an adapter-dimer pair is one of these): nothing here;
+ *   only read 1 passes: with an unpaired-1 writer, read 1 to unpaired1 and read 2 to failed with its reason; without one, failed gets
+ *       read 1 tagged "paired_read_is_failing", then read 2 with its reason;
+ *   only read 2 passes: with an unpaired-2 writer, read 2 to unpaired2 and read 1 to failed with its reason; otherwise, with an unpaired-1
+ *       writer, read 2 to unpaired1 and read 1 to failed; otherwise failed gets read 1 with its reason, then read 2 tagged
+ *       "paired_read_is_failing".
+ * A failed record is Read::appendToStringWithTag (src/read.cpp:136-154): the name line, ' ', the tag of FAILED_TYPES (src/common.h:56-65:
+ * failed_too_many_n_bases, failed_too_short, failed_too_long, failed_quality_filter, failed_low_complexity, failed_adapter_dimer),
+ * then sequence, strand and quality lines.  The read written is the one trimAndCut changed in place: its kept window with any corrected
+ * bases; a read trimAndCut dropped (FP_F_DROPPED) was never touched and is written whole, row bytes [0, decoded length).  Unpaired
+ * records are written like out1 / out2.  A tagged record is at most 24 bytes longer than the input record.
+ * Writers: the reference's --unpaired2 defaults to --unpaired1 and is a writer of its own only when the two names differ
+ * (src/main.cpp:188-189, src/peprocessor.cpp:68-72).  Its CLI hands the unpaired-2 text to a file only when both writers exist (:681-686);
+ * the library returns it whenever FP_FQ_W_UNPAIRED2 is set and leaves that choice to the caller.
+ * fp_fastq_encode_rejects writes ONE stream of a batch the chain has worked on, all pointers DEVICE (side 2 NULL for single-end):
+ *   which                FP_FQ_OUT_UNPAIRED1 / _UNPAIRED2 (paired only) or FP_FQ_OUT_FAILED
+ *   writers              FP_FQ_W_* of the unpaired writers that exist (0 for single-end)
+ *   d_text*, d_recs*     as fp_fastq_encode_merge; d_res* what fp_process_se / _pe wrote (the merging branch is read off FP_F_MERGED)
+ *   d_seq*, d_qual*      the rows as the chain left them; d_len* the decoded lengths (fp_fastq_decode's d_len; the chain does not change them)
+ *   n, d_out, out_cap, out_bytes  as fp_fastq_encode.
+ * FP_E_INVAL: unpaired stream or writers on a single-end ctx, writers on a ctx with merge_enabled and merge_include_unmerged (the reference
+ * ignores both options there, src/options.cpp:136-143,222-229).  Synchronous. */
+#define FP_FQ_OUT_UNPAIRED1 3
+#define FP_FQ_OUT_UNPAIRED2 4
+#define FP_FQ_OUT_FAILED    5
+#define FP_FQ_OUTS          6
+#define FP_FQ_W_UNPAIRED1   0x1
+#define FP_FQ_W_UNPAIRED2   0x2
+int  fp_fastq_encode_rejects(fp_ctx* ctx, int32_t which, int32_t writers, const uint8_t* d_text1, const fp_fastq_rec* d_recs1,
+                             const uint8_t* d_text2, const fp_fastq_rec* d_recs2, const fp_read_result* d_res1, const fp_read_result* d_res2,
+                             const uint8_t* d_seq1, const uint8_t* d_qual1, const uint16_t* d_len1,
+                             const uint8_t* d_seq2, const uint8_t* d_qual2, const uint16_t* d_len2,
+                             int64_t n, uint8_t* d_out, int64_t out_cap, int64_t* out_bytes);
+/* The text path with every output stream: outs / out_caps / out_bytes are indexed by FP_FQ_OUT_* (merged, out1, out2, unpaired1, unpaired2,
+ * failed).  A NULL buffer is not wanted; a NULL unpaired buffer also means that writer does not exist, which decides where reads go (above).
+ * Works for single-end, paired and merging ctxs; out_bytes[k] is set for every k.  FP_E_INVAL, touching nothing: an unpaired buffer on a
+ * single-end ctx or with merge_include_unmerged, a merged buffer on a ctx that does not merge, an out2 buffer on a single-end ctx.
+ * FP_E_TOOLARGE when a stream outgrows its buffer, as for fp_fastq_process_host.  Everything else is fp_fastq_process_host(_merge). */
+int  fp_fastq_process_host_outs(fp_ctx* ctx, const uint8_t* text1, int64_t nbytes1, const uint8_t* text2, int64_t nbytes2,
+                                int32_t final_chunk, int32_t phred64, uint8_t* const outs[FP_FQ_OUTS], const int64_t out_caps[FP_FQ_OUTS],
+                                int64_t out_bytes[FP_FQ_OUTS], int64_t* n_units, int64_t* consumed1, int64_t* consumed2,
+                                fp_fastq_info* info1, fp_fastq_info* info2);
+
 /* ---------------- duplication bloom filter (SURVEY.md 8(f) rank 2; src/duplicate.cpp) ----------------
  * fp_dup_check replaces Duplicate::checkRead / checkPair (src/duplicate.cpp:126-154) for a batch in DEVICE memory: d_is_dup[i]
  * (nullable) = what the reference returns for unit i when units are fed in index order, batch after batch -- deterministic, not
