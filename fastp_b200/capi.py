@@ -188,6 +188,10 @@ SYMBOLS = {
                                              C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
                                              C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
                                              C.POINTER(FastqInfo), C.POINTER(FastqInfo)]),
+    "fp_fastq_decode_interleaved": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32] + [C.c_void_p] * 8
+                                    + [C.c_int64, C.POINTER(FastqInfo)]),
+    "fp_fastq_encode_interleaved": (C.c_int, [C.c_void_p] + [C.c_void_p] * 10 + [C.c_int64, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]),
+    "fp_fastq_set_interleaved": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
 }
 
 

@@ -121,6 +121,7 @@ struct fp_ctx {
     int64_t dup_total = 0;
     const uint8_t* dup_flags = nullptr;     /* fp_set_dup_flags: --dedup flags of the batch the next launch works on */
     int fq_dup_level = 0, fq_dedup = 0;     /* fp_fastq_set_dedup */
+    int fq_il_in = 0, fq_il_out = 0;        /* fp_fastq_set_interleaved */
     Buf fq_dupflags;
     Buf dup_pos, dup_keys, dup_vals;
     /* kernel timing */
@@ -1297,13 +1298,15 @@ static int fq_ensure(fp_ctx::Buf& b, size_t need) {
 
 static_assert(sizeof(fp_fastq_rec) == sizeof(fq_rec), "fp_fastq_rec layout");
 
-/* rec_end_out (optional, host): consumed bytes if only the first k records are kept is read later through fq_recend */
+/* rec_end_out (optional, host): consumed bytes if only the first k records are kept is read later through fq_recend.
+   il: interleaved text, mate 1 rows in d_seq .. d_recs and mate 2 rows in il's side 1; capacity and info->n_records count pairs. */
 static int fastq_decode_impl(fp_ctx* c, const uint8_t* d_text, int64_t nbytes, int32_t final_chunk, int32_t phred64,
                              uint8_t* d_seq, uint8_t* d_qual, uint16_t* d_len, int64_t capacity, fp_fastq_rec* d_recs,
-                             fp_fastq_info* info, fp_ctx::Buf& recend) {
+                             fp_fastq_info* info, fp_ctx::Buf& recend, const fq_side_rows* il = nullptr) {
     if (!c || !info || (nbytes > 0 && !d_text)) return set_err(FP_E_INVAL, "null argument");
     if (nbytes < 0 || nbytes >= ((int64_t)1 << 32) - 16) return set_err(FP_E_TOOLARGE, "FASTQ chunk must be smaller than 4 GiB");
     if (capacity < 0 || (capacity > 0 && (!d_seq || !d_qual || !d_len || !d_recs))) return set_err(FP_E_INVAL, "null row buffers");
+    if (il && capacity > 0 && (!il->seq[1] || !il->qual[1] || !il->len[1] || !il->recs[1])) return set_err(FP_E_INVAL, "null row buffers");
     memset(info, 0, sizeof(*info));
     info->error_record = -1;
     if (nbytes == 0) return FP_OK;
@@ -1343,15 +1346,25 @@ static int fastq_decode_impl(fp_ctx* c, const uint8_t* d_text, int64_t nbytes, i
     if (nstarted > 0)
         fq_fsm_kernel<1><<<nlb, FQ_T, 0, st>>>(d_text, nbytes, d_term, nlines, nullptr, (const unsigned int*)c->fq_bstate.p, (const unsigned int*)c->fq_brec.p,
                                                d_recline, nstarted);
-    const unsigned int nrec = (unsigned int)std::min<int64_t>(ncomplete, capacity);
+    const unsigned int nrec = (unsigned int)std::min<int64_t>(ncomplete, il ? 2 * capacity : capacity);
+    fq_side_rows S{};
+    if (il) { S = *il; S.seq[0] = d_seq; S.qual[0] = d_qual; S.len[0] = d_len; S.recs[0] = reinterpret_cast<fq_rec*>(d_recs); }
     if (nrec > 0) {
         if ((rc = fq_ensure(recend, (size_t)nrec * 4))) return rc;
         CK(cudaMemsetAsync(d_info + 8, 0xFF, 4, st));             /* first bad record = none */
-        fq_scatter_kernel<<<(nrec + FQ_T / 32 - 1) / (FQ_T / 32), FQ_T, 0, st>>>(d_text, nbytes, d_term, d_recline, nrec, c->stride, phred64,
-                                                                                   d_seq, d_qual, d_len, reinterpret_cast<fq_rec*>(d_recs),
-                                                                                   (unsigned int*)recend.p, d_info + 8, d_info + 9);
+        if (il)
+            fq_scatter_il_kernel<<<(nrec + FQ_T / 32 - 1) / (FQ_T / 32), FQ_T, 0, st>>>(d_text, nbytes, d_term, d_recline, nrec, c->stride, phred64, S,
+                                                                                          (unsigned int*)recend.p, d_info + 8, d_info + 9);
+        else
+            fq_scatter_kernel<<<(nrec + FQ_T / 32 - 1) / (FQ_T / 32), FQ_T, 0, st>>>(d_text, nbytes, d_term, d_recline, nrec, c->stride, phred64,
+                                                                                       d_seq, d_qual, d_len, reinterpret_cast<fq_rec*>(d_recs),
+                                                                                       (unsigned int*)recend.p, d_info + 8, d_info + 9);
     }
-    fq_finish_kernel<<<1, 1, 0, st>>>(d_term, nlines, nterm, nbytes, d_recline, nstarted, ncomplete, nrec, reinterpret_cast<const fq_rec*>(d_recs), d_info + 8, m_info + 8);
+    if (il)
+        fq_finish_il_kernel<<<1, 1, 0, st>>>(d_term, nlines, nterm, nbytes, final_chunk, d_recline, nstarted, ncomplete, nrec, S.recs[0], S.recs[1],
+                                             d_info + 8, m_info + 8);
+    else
+        fq_finish_kernel<<<1, 1, 0, st>>>(d_term, nlines, nterm, nbytes, d_recline, nstarted, ncomplete, nrec, reinterpret_cast<const fq_rec*>(d_recs), d_info + 8, m_info + 8);
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(st));
     info->n_records = h_info[8];
@@ -1367,6 +1380,17 @@ extern "C" int fp_fastq_decode(fp_ctx* c, const uint8_t* d_text, int64_t nbytes,
                                fp_fastq_info* info) {
     if (!c) return set_err(FP_E_INVAL, "null argument");
     return fastq_decode_impl(c, d_text, nbytes, final_chunk, phred64, d_seq, d_qual, d_len, capacity, d_recs, info, c->fq_recend);
+}
+
+extern "C" int fp_fastq_decode_interleaved(fp_ctx* c, const uint8_t* d_text, int64_t nbytes, int32_t final_chunk, int32_t phred64,
+                                           uint8_t* d_seq1, uint8_t* d_qual1, uint16_t* d_len1, fp_fastq_rec* d_recs1,
+                                           uint8_t* d_seq2, uint8_t* d_qual2, uint16_t* d_len2, fp_fastq_rec* d_recs2,
+                                           int64_t capacity, fp_fastq_info* info) {
+    if (!c) return set_err(FP_E_INVAL, "null argument");
+    if (capacity >= ((int64_t)1 << 30)) return set_err(FP_E_TOOLARGE, "capacity must be below 2^30 pairs");
+    fq_side_rows il{};
+    il.seq[1] = d_seq2; il.qual[1] = d_qual2; il.len[1] = d_len2; il.recs[1] = reinterpret_cast<fq_rec*>(d_recs2);
+    return fastq_decode_impl(c, d_text, nbytes, final_chunk, phred64, d_seq1, d_qual1, d_len1, capacity, d_recs1, info, c->fq_recend, &il);
 }
 
 /* size pass, scan and write pass of one output stream (fp_fastq.cuh); M is unused by FQ_SEL_PLAIN */
@@ -1397,6 +1421,22 @@ extern "C" int fp_fastq_encode(fp_ctx* c, const uint8_t* d_text, const fp_fastq_
     if (n <= 0) return FP_OK;
     if (!d_text || !d_recs || !d_res || !d_seq || !d_qual || (out_cap > 0 && !d_out)) return set_err(FP_E_INVAL, "null argument");
     return fastq_encode_impl<FQ_SEL_PLAIN>(c, d_text, d_recs, d_res, d_seq, d_qual, fq_merge_args{}, n, d_out, out_cap, out_bytes);
+}
+
+extern "C" int fp_fastq_encode_interleaved(fp_ctx* c, const uint8_t* d_text1, const fp_fastq_rec* d_recs1, const uint8_t* d_text2, const fp_fastq_rec* d_recs2,
+                                           const fp_read_result* d_res1, const fp_read_result* d_res2,
+                                           const uint8_t* d_seq1, const uint8_t* d_qual1, const uint8_t* d_seq2, const uint8_t* d_qual2,
+                                           int64_t n, uint8_t* d_out, int64_t out_cap, int64_t* out_bytes) {
+    if (!c || !out_bytes) return set_err(FP_E_INVAL, "null argument");
+    *out_bytes = 0;
+    if (!c->p.paired) return set_err(FP_E_INVAL, "ctx was created for single-end data: interleaved output needs pairs");
+    if (c->p.merge_enabled) return set_err(FP_E_INVAL, "ctx merges pairs: its stdout stream is the merged one (fp_fastq_encode_merge)");
+    if (n <= 0) return FP_OK;
+    if (!d_text1 || !d_recs1 || !d_text2 || !d_recs2 || !d_res1 || !d_res2 || !d_seq1 || !d_qual1 || !d_seq2 || !d_qual2 || (out_cap > 0 && !d_out))
+        return set_err(FP_E_INVAL, "null argument");
+    fq_merge_args M{};
+    M.text2 = d_text2; M.recs2 = reinterpret_cast<const fq_rec*>(d_recs2); M.res2 = d_res2; M.seq2 = d_seq2; M.qual2 = d_qual2;
+    return fastq_encode_impl<FQ_SEL_INTERLEAVED>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
 }
 
 extern "C" int fp_fastq_encode_merge(fp_ctx* c, int32_t which, const uint8_t* d_text1, const fp_fastq_rec* d_recs1, const uint8_t* d_text2, const fp_fastq_rec* d_recs2,
@@ -1466,7 +1506,11 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
     const int sides = c->p.paired ? 2 : 1;
     const bool merging = c->p.merge_enabled && sides == 2;
     const int writers = (outs[FP_FQ_OUT_UNPAIRED1] ? FP_FQ_W_UNPAIRED1 : 0) | (outs[FP_FQ_OUT_UNPAIRED2] ? FP_FQ_W_UNPAIRED2 : 0);
+    /* fp_fastq_set_interleaved: mates alternate in text1 (one upload, one decode per round); out1 receives read 1 and read 2 of every pair */
+    const bool il_in = c->fq_il_in && sides == 2, il_out = c->fq_il_out && sides == 2 && !merging;
     if (c->dup_flags) return set_err(FP_E_INVAL, "duplicate flags are set (fp_set_dup_flags): the text path runs its own duplicate filter (fp_fastq_set_dedup)");
+    if (il_in && (text2 || nbytes2 != 0)) return set_err(FP_E_INVAL, "interleaved input: both mates are in text1 (pass text2 NULL and nbytes2 0)");
+    if (il_out && outs[FP_FQ_OUT_R2]) return set_err(FP_E_INVAL, "interleaved output: both reads go to out1 (pass no out2 buffer)");
     CK(cudaSetDevice(c->device));
     cudaStream_t st = c->stream[0], up = c->stream[1];
     if (!c->fq_stream_out) {
@@ -1476,7 +1520,7 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
     }
     cudaStream_t outst = c->fq_stream_out;
     const uint8_t* text[2] = {text1, text2};
-    const int64_t nb[2] = {nbytes1, sides == 2 ? nbytes2 : 0};
+    const int64_t nb[2] = {nbytes1, sides == 2 && !il_in ? nbytes2 : 0};
     const int64_t cap = c->max_batch;
     /* The text goes up in pieces on its own stream while the pieces already on the device are decoded, run through the chain and
        encoded, and the previous round's output text goes down on a third stream: H2D, kernels and D2H overlap inside ONE call
@@ -1517,17 +1561,22 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
         if ((rc = upload_more())) return rc;                      /* ... while the next piece flies */
         fp_fastq_info inf[2]; memset(inf, 0, sizeof(inf));
         int fin[2];
-        for (int s = 0; s < sides; s++) {
+        fq_side_rows il{};
+        il.seq[1] = (uint8_t*)c->fqh_seq[1].p; il.qual[1] = (uint8_t*)c->fqh_qual[1].p; il.len[1] = (uint16_t*)c->fqh_len[1].p;
+        il.recs[1] = (fq_rec*)c->fqh_recs[1].p;
+        const int decodes = il_in ? 1 : sides;
+        for (int s = 0; s < decodes; s++) {
             fin[s] = (final_chunk && have[s] >= nb[s]) ? 1 : 0;
             rc = fastq_decode_impl(c, (const uint8_t*)c->fqh_text[s].p + rstart[s], have[s] - rstart[s], fin[s], phred64, (uint8_t*)c->fqh_seq[s].p,
-                                   (uint8_t*)c->fqh_qual[s].p, (uint16_t*)c->fqh_len[s].p, cap, (fp_fastq_rec*)c->fqh_recs[s].p, &inf[s], c->fqh_recend[s]);
+                                   (uint8_t*)c->fqh_qual[s].p, (uint16_t*)c->fqh_len[s].p, cap, (fp_fastq_rec*)c->fqh_recs[s].p, &inf[s], c->fqh_recend[s],
+                                   il_in ? &il : nullptr);
             if (rc) return rc;
         }
         const double t1 = now();
         int64_t n = inf[0].n_records;
-        if (sides == 2) n = std::min(n, inf[1].n_records);        /* pairs end with the shorter input (FastqReaderPair::read) */
+        if (sides == 2 && !il_in) n = std::min(n, inf[1].n_records);   /* pairs end with the shorter input (FastqReaderPair::read) */
         bool reader_ended = false;                                /* a reader hit a record it rejects: it returns NULL, the stream ends */
-        for (int s = 0; s < sides; s++) {
+        for (int s = 0; s < decodes; s++) {
             int64_t used = inf[s].consumed;
             if (n != inf[s].n_records) {                          /* this side decoded more records than the pair count: keep only n */
                 used = 0;                                         /* resume right after record n-1 (end offsets were kept per side) */
@@ -1562,13 +1611,14 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
             if (rc) return rc;
             CK(cudaEventSynchronize(c->fq_ev_out[flip]));        /* the output buffers of two rounds ago have gone down */
             const uint8_t* rtext[2] = {(const uint8_t*)c->fqh_text[0].p + rstart[0], sides == 2 ? (const uint8_t*)c->fqh_text[1].p + rstart[1] : nullptr};
+            if (il_in) rtext[1] = rtext[0];                       /* both mates' records point into the one text */
             for (int s = 0; s < FP_FQ_OUTS; s++) {
                 if (!outs[s]) continue;                           /* caller does not want this stream's text */
                 fp_ctx::Buf& ob = c->fqh_outbuf[flip][s];
                 const int64_t room = std::max<int64_t>(ocap[s] - obytes[s], 0);
                 /* per unit: one record of a side; on the merged stream one read of up to two rows, or two records; on the failed stream two
                    tagged records */
-                const bool two = s == FP_FQ_OUT_MERGED || s == FP_FQ_OUT_FAILED;
+                const bool two = s == FP_FQ_OUT_MERGED || s == FP_FQ_OUT_FAILED || (il_out && s == FP_FQ_OUT_R1);
                 int64_t want = std::min<int64_t>(room, n * (int64_t)(two ? 4 * c->stride + 512 : 2 * c->stride + 256));
                 int64_t total = 0;
                 const fp_fastq_rec* recs[2] = {(const fp_fastq_rec*)c->fqh_recs[0].p, (const fp_fastq_rec*)c->fqh_recs[1].p};
@@ -1581,6 +1631,9 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
                         rc = fp_fastq_encode_rejects(c, s, writers, rtext[0], recs[0], rtext[1], recs[1], res[0], res[1], seq[0], qual[0],
                                                      (const uint16_t*)c->fqh_len[0].p, seq[1], qual[1], (const uint16_t*)c->fqh_len[1].p,
                                                      n, (uint8_t*)ob.p, want, &total);
+                    else if (il_out)                              /* s == FP_FQ_OUT_R1: an out2 buffer was refused above */
+                        rc = fp_fastq_encode_interleaved(c, rtext[0], recs[0], rtext[1], recs[1], res[0], res[1], seq[0], qual[0], seq[1], qual[1],
+                                                         n, (uint8_t*)ob.p, want, &total);
                     else if (merging)
                         rc = fp_fastq_encode_merge(c, s, rtext[0], recs[0], rtext[1], recs[1], res[0], res[1], (const fp_ov_result*)c->fqh_ov.p,
                                                    seq[0], qual[0], seq[1], qual[1], n, (uint8_t*)ob.p, want, &total);
@@ -1610,6 +1663,7 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
     CK(cudaStreamSynchronize(outst));
     if (trace) fprintf(stderr, "[fq] loop %.2f ms, drain %.2f ms\n", t_loop - t_begin, now() - t_loop);
     agg[0].consumed = start[0]; agg[1].consumed = start[1];
+    if (il_in) memset(&agg[1], 0, sizeof(agg[1]));
     *n_units = units; *consumed1 = start[0]; if (consumed2) *consumed2 = start[1];
     for (int s = 0; s < FP_FQ_OUTS; s++) if (out_bytes[s]) *out_bytes[s] = obytes[s];
     if (info1) *info1 = agg[0];
@@ -1722,6 +1776,15 @@ extern "C" int fp_fastq_set_dedup(fp_ctx* c, int32_t accuracy_level, int32_t ded
     if (!c) return set_err(FP_E_INVAL, "null argument");
     if (accuracy_level < 0 || accuracy_level > 6) return set_err(FP_E_INVAL, "dup accuracy level must be 0 (off) .. 6");
     c->fq_dup_level = accuracy_level; c->fq_dedup = dedup ? 1 : 0;
+    return FP_OK;
+}
+
+extern "C" int fp_fastq_set_interleaved(fp_ctx* c, int32_t in, int32_t out) {
+    if (!c) return set_err(FP_E_INVAL, "null argument");
+    if (in && !c->p.paired) return set_err(FP_E_INVAL, "interleaved input needs a paired ctx");
+    if (out && !c->p.paired) return set_err(FP_E_INVAL, "interleaved output needs a paired ctx");
+    if (out && c->p.merge_enabled) return set_err(FP_E_INVAL, "interleaved output on a ctx that merges pairs (its stdout stream is the merged one)");
+    c->fq_il_in = in ? 1 : 0; c->fq_il_out = out ? 1 : 0;
     return FP_OK;
 }
 

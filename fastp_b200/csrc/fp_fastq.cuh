@@ -237,14 +237,35 @@ __global__ void fq_fsm_scan_kernel(const fq_elem* block_agg, int nblocks, unsign
     info[3] = (st == 0) ? rec : (rec > 0 ? rec - 1 : 0);
 }
 
-/* ---- scatter: one warp per record ---- */
+/* ---- scatter: one warp per record ----
+ * record r of the text goes to row `row`; first_bad / rec_end are indexed by r */
+__device__ __forceinline__ void fq_scatter_record(const uint8_t* text, long long n, const unsigned int* term, const unsigned int* rec_line,
+                                                  unsigned int r, unsigned int row, int stride, int phred64,
+                                                  uint8_t* seq, uint8_t* qual, uint16_t* len, fq_rec* recs,
+                                                  unsigned int* rec_end, unsigned int* first_bad, unsigned int* bad_code, int lane);
 __global__ void __launch_bounds__(FQ_T) fq_scatter_kernel(const uint8_t* text, long long n, const unsigned int* term, const unsigned int* rec_line,
                                                           unsigned int nrec, int stride, int phred64,
                                                           uint8_t* seq, uint8_t* qual, uint16_t* len, fq_rec* recs,
                                                           unsigned int* rec_end, unsigned int* first_bad, unsigned int* bad_code) {
     const unsigned int r = blockIdx.x * (FQ_T / 32) + (threadIdx.x >> 5);
-    const int lane = threadIdx.x & 31;
     if (r >= nrec) return;
+    fq_scatter_record(text, n, term, rec_line, r, r, stride, phred64, seq, qual, len, recs, rec_end, first_bad, bad_code, threadIdx.x & 31);
+}
+/* interleaved text (--interleaved_in, FastqReaderPair::read src/fastqreader.cpp:452-460): record r is mate (r & 1) of pair r >> 1 */
+struct fq_side_rows { uint8_t* seq[2]; uint8_t* qual[2]; uint16_t* len[2]; fq_rec* recs[2]; };
+__global__ void __launch_bounds__(FQ_T) fq_scatter_il_kernel(const uint8_t* text, long long n, const unsigned int* term, const unsigned int* rec_line,
+                                                             unsigned int nrec, int stride, int phred64, fq_side_rows S,
+                                                             unsigned int* rec_end, unsigned int* first_bad, unsigned int* bad_code) {
+    const unsigned int r = blockIdx.x * (FQ_T / 32) + (threadIdx.x >> 5);
+    if (r >= nrec) return;
+    const bool m2 = r & 1;                                      /* selects, not indexes: S stays in parameter space */
+    fq_scatter_record(text, n, term, rec_line, r, r >> 1, stride, phred64, m2 ? S.seq[1] : S.seq[0], m2 ? S.qual[1] : S.qual[0],
+                      m2 ? S.len[1] : S.len[0], m2 ? S.recs[1] : S.recs[0], rec_end, first_bad, bad_code, threadIdx.x & 31);
+}
+__device__ __forceinline__ void fq_scatter_record(const uint8_t* text, long long n, const unsigned int* term, const unsigned int* rec_line,
+                                                  unsigned int r, unsigned int row, int stride, int phred64,
+                                                  uint8_t* seq, uint8_t* qual, uint16_t* len, fq_rec* recs,
+                                                  unsigned int* rec_end, unsigned int* first_bad, unsigned int* bad_code, int lane) {
     const unsigned int l = rec_line[r];
     unsigned int ns, ne, ss, se, ps, pe, qs, qe;
     fq_line_span(text, n, term, l, ns, ne);
@@ -260,7 +281,7 @@ __global__ void __launch_bounds__(FQ_T) fq_scatter_kernel(const uint8_t* text, l
         /* a later, smaller r may overwrite the code again: the host re-reads the code of first_bad through rec codes below */
     }
     const int L = code == FQ_ERR_NONE ? (int)(se - ss) : 0;
-    uint8_t* srow = seq + (size_t)r * stride; uint8_t* qrow = qual + (size_t)r * stride;
+    uint8_t* srow = seq + (size_t)row * stride; uint8_t* qrow = qual + (size_t)row * stride;
     for (int i = lane; i < stride; i += 32) {
         uint8_t b = 0, q = 0;
         if (i < L) {
@@ -270,13 +291,13 @@ __global__ void __launch_bounds__(FQ_T) fq_scatter_kernel(const uint8_t* text, l
         srow[i] = b; qrow[i] = q;
     }
     if (lane == 0) {
-        len[r] = (uint16_t)L;
+        len[row] = (uint16_t)L;
         fq_rec rc; rc.name_off = ns; rc.name_len = ne - ns; rc.strand_off = ps; rc.strand_len = pe - ps;
-        recs[r] = rc;
+        recs[row] = rc;
         /* first byte after this record's quality line (and its terminator) */
         const unsigned int t = term[l + 3];
         rec_end[r] = (long long)t < n ? t + 1u : (unsigned int)n;
-        if (code != FQ_ERR_NONE) recs[r].name_len |= 0x80000000u | ((unsigned int)code << 28);     /* marks the record as bad */
+        if (code != FQ_ERR_NONE) recs[row].name_len |= 0x80000000u | ((unsigned int)code << 28);     /* marks the record as bad */
     }
 }
 
@@ -302,6 +323,31 @@ __global__ void fq_finish_kernel(const unsigned int* term, unsigned int nlines, 
     out[0] = keep; out[1] = err; out[2] = fb; out[3] = more;
     out[4] = (unsigned int)(consumed & 0xFFFFFFFFll); out[5] = (unsigned int)(consumed >> 32);
 }
+/* fq_finish_kernel for interleaved text: out[0] counts PAIRS, out[2] is the first bad record's index in the text.  nrec (records
+ * scattered) is even whenever capacity cut it.  The reference's pair stream ends at the first NULL of either mate (ReadPair::eof,
+ * src/read.cpp:203-205), so a bad mate 2 also drops the good mate 1 before it, and a lone last record is dropped without a message. */
+__global__ void fq_finish_il_kernel(const unsigned int* term, unsigned int nlines, unsigned int nterm, long long nbytes, int final_chunk,
+                                    const unsigned int* rec_line, unsigned int nstarted, unsigned int ncomplete, unsigned int nrec,
+                                    const fq_rec* recs1, const fq_rec* recs2, const unsigned int* first_bad, unsigned int* out) {
+    if (blockIdx.x || threadIdx.x) return;
+    const unsigned int fb = nrec > 0 ? *first_bad : 0xFFFFFFFFu;
+    unsigned int keep = nrec >> 1, err = FQ_ERR_NONE, more = 0;
+    long long consumed;
+    auto line_start = [&](unsigned int l) -> long long { return l == 0 ? 0ll : (long long)term[l - 1] + 1; };
+    if (fb != 0xFFFFFFFFu) {
+        err = (((fb & 1u) ? recs2 : recs1)[fb >> 1].name_len >> 28) & 7u; keep = fb >> 1; consumed = nbytes;
+    } else if (ncomplete > nrec) {                             /* capacity (in pairs) reached: resume at record 2 * capacity */
+        more = 1; consumed = line_start(rec_line[nrec]);
+    } else if (nrec & 1u) {                                    /* a lone mate 1: dropped at the end of the input, else read again with its mate */
+        consumed = final_chunk ? nbytes : line_start(rec_line[nrec - 1]);
+    } else if (nstarted > ncomplete) {
+        consumed = line_start(rec_line[ncomplete]);
+    } else {
+        consumed = nlines > nterm ? nbytes : (long long)term[nlines - 1] + 1;
+    }
+    out[0] = keep; out[1] = err; out[2] = fb; out[3] = more;
+    out[4] = (unsigned int)(consumed & 0xFFFFFFFFll); out[5] = (unsigned int)(consumed >> 32);
+}
 __global__ void fq_set_u32_kernel(unsigned int* p, unsigned int v) { if (!blockIdx.x && !threadIdx.x) *p = v; }
 __global__ void fq_copy_u32_kernel(const unsigned int* src, unsigned int* dst) { if (!blockIdx.x && !threadIdx.x) *dst = *src; }
 
@@ -315,6 +361,8 @@ __global__ void fq_copy_u32_kernel(const unsigned int* src, unsigned int* dst) {
  *                  --unpaired1 / --unpaired2 / --failed_out: what a unit that is not a flagged duplicate, and that took neither merging
  *                  branch, writes when exactly one read passes (peprocessor.cpp:594-620), or SE when the read fails (seprocessor.cpp:287-289);
  *                  see fq_reject_plan
+ *   FQ_SEL_INTERLEAVED  --stdout for pairs (peprocessor.cpp:579-581, singleOutput): for every unit, read 1's record as FQ_SEL_PLAIN writes
+ *                  it on out1, then read 2's as it writes it on out2 -- out1 and out2 interleaved record by record
  * The primary arrays (text, recs, res, seq, qual) are read 1's for FQ_SEL_MERGED and the reject streams, and the written side's for
  * FQ_SEL_SIDE; fq_merge_args carries the other side (FQ_SEL_SIDE reads only its records). */
 #define FQ_SCAN_ITEMS 2048
@@ -324,6 +372,7 @@ __global__ void fq_copy_u32_kernel(const unsigned int* src, unsigned int* dst) {
 #define FQ_SEL_UNPAIRED1 3
 #define FQ_SEL_UNPAIRED2 4
 #define FQ_SEL_FAILED 5
+#define FQ_SEL_INTERLEAVED 6
 struct fq_merge_args {
     const uint8_t* text2; const fq_rec* recs2; const fp_read_result* res2; const uint8_t* seq2; const uint8_t* qual2;
     const fp_ov_result* ov;
@@ -469,6 +518,10 @@ __device__ __forceinline__ unsigned long long fq_write_reject(uint8_t* d, const 
 /* bytes unit i puts on the selected stream */
 template <int SEL>
 __device__ __forceinline__ unsigned long long fq_unit_size(const uint8_t* text, const fq_rec* recs, const fp_read_result* res, const fq_merge_args& M, long long i) {
+    if (SEL == FQ_SEL_INTERLEAVED) {
+        const fp_read_result a = res[i], b = M.res2[i];
+        return (fq_written(a, a.pair_verdict) ? fq_record_size(recs[i], a) : 0ull) + (fq_written(b, b.pair_verdict) ? fq_record_size(M.recs2[i], b) : 0ull);
+    }
     if (SEL >= FQ_SEL_UNPAIRED1) return fq_reject_size<SEL>(recs, res, M, i);
     const fp_read_result r = res[i];
     if (SEL == FQ_SEL_PLAIN) return fq_written(r, r.pair_verdict) ? fq_record_size(recs[i], r) : 0ull;
@@ -583,6 +636,17 @@ __global__ void __launch_bounds__(FQ_T) fq_encode_kernel(const uint8_t* text, co
             const unsigned long long o = s_sz[j];
             if (need == 0 || o + need > out_cap) continue;            /* a unit that does not fit is skipped whole: caller sees total > cap */
             uint8_t* d = out + o;
+            if (SEL == FQ_SEL_INTERLEAVED) {                           /* read 1 then read 2, each under its own side's rule */
+                const size_t row = (size_t)ri * stride;
+                const fp_read_result b = M.res2[ri];                 /* read 2's record ends the unit's `need` bytes */
+                if (fq_written(b, b.pair_verdict)) {
+                    const fq_rec rc2 = M.recs2[ri];
+                    fq_write_record(d + (need - fq_record_size(rc2, b)), M.text2, rc2, b, M.seq2 + row, M.qual2 + row, lane);
+                }
+                const fp_read_result a = res[ri];
+                if (fq_written(a, a.pair_verdict)) fq_write_record(d, text, recs[ri], a, seq + row, qual + row, lane);
+                continue;
+            }
             if (SEL >= FQ_SEL_UNPAIRED1) {                             /* reject streams: the unit's records in plan order */
                 const unsigned int P = fq_reject_plan<SEL>(res[ri], M, ri);
                 d += fq_write_reject(d, text, recs, res, seq, qual, M, fq_plan_side(P, 0), fq_plan_tag(P, 0), stride, ri, lane);

@@ -105,6 +105,12 @@ public:
     bool inputEnded() const { return mInputEnded; }
     /* text path: Duplicate::checkRead / checkPair on the device at `accuracyLevel` (src/main.cpp:200-209; 0 = off); dedup: drop duplicates (-D) */
     bool setDedup(int accuracyLevel, bool dedup) { return mCtx && fp_fastq_set_dedup(mCtx, accuracyLevel, dedup ? 1 : 0) == FP_OK; }
+    /* text path, paired runs: in = mates alternate in text1 (--interleaved_in; pass text2 NULL, n2 0), out = outstr1 receives read 1 then read 2
+     * of every pair (--stdout, src/peprocessor.cpp:579-581; not with merging, whose stdout stream is `merged`) and outstr2 nothing */
+    bool setInterleaved(bool in, bool out) {
+        if (!mCtx || fp_fastq_set_interleaved(mCtx, in ? 1 : 0, out ? 1 : 0) != FP_OK) return false;
+        mIlIn = in; mIlOut = out; return true;
+    }
     bool dupTotals(long* total, long* dups) { int64_t t = 0, d = 0; if (!mCtx || fp_dup_totals(mCtx, &t, &d) != FP_OK) return false; *total = (long)t; *dups = (long)d; return true; }
     bool processFastqText(const char* text1, size_t n1, const char* text2, size_t n2, bool final, bool phred64,
                           std::string* outstr1, std::string* outstr2, size_t* consumed1, size_t* consumed2, long* units,
@@ -129,6 +135,7 @@ private:
     fp_ov_result* mOv = nullptr;
     std::vector<uint8_t> mTextOut[FP_FQ_OUTS];      /* indexed by FP_FQ_OUT_*: merged, out1, out2, unpaired1, unpaired2, failed */
     bool mInputEnded = false;
+    bool mIlIn = false, mIlOut = false;
     std::string mError;
 };
 

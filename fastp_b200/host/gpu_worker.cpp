@@ -177,16 +177,20 @@ bool GpuChainWorker::processFastqText(const char* text1, size_t n1, const char* 
                                       std::string* outstr1, std::string* outstr2, size_t* consumed1, size_t* consumed2, long* units,
                                       std::string* merged, std::string* unpaired1, std::string* unpaired2, std::string* failed) {
     const bool paired = mParams.paired != 0, merging = paired && mParams.merge_enabled;
+    const bool ilIn = paired && mIlIn, ilOut = paired && mIlOut;
+    if (ilIn) n2 = 0;                                           /* both mates are in text1 */
     int64_t nu = 0, c1 = 0, c2 = 0;
     fp_fastq_info i1, i2;
-    const uint8_t* t1 = reinterpret_cast<const uint8_t*>(text1); const uint8_t* t2 = paired ? reinterpret_cast<const uint8_t*>(text2) : nullptr;
+    const uint8_t* t1 = reinterpret_cast<const uint8_t*>(text1); const uint8_t* t2 = paired && !ilIn ? reinterpret_cast<const uint8_t*>(text2) : nullptr;
     const size_t both = n1 + (paired ? n2 : 0);
-    /* what each stream can hold at most: a side's reads; on the merged stream everything both inputs hold, each merged read with its name
-       suffix (one per pair, i.e. per 8 lines at least); on unpaired1 reads of either side; on the failed stream reads of either side, each
-       with a tag of up to 24 bytes (a record takes 6 bytes at least) */
-    std::string* want[FP_FQ_OUTS] = {merging ? merged : nullptr, outstr1, paired ? outstr2 : nullptr, paired ? unpaired1 : nullptr,
+    const size_t side2 = ilIn ? n1 : n2;                        /* the text that holds read 2 */
+    /* what each stream can hold at most: a side's reads (both sides' when interleaved); on the merged stream everything both inputs hold, each
+       merged read with its name suffix (one per pair, i.e. per 8 lines at least); on unpaired1 reads of either side; on the failed stream
+       reads of either side, each with a tag of up to 24 bytes (a record takes 6 bytes at least) */
+    std::string* want[FP_FQ_OUTS] = {merging ? merged : nullptr, outstr1, paired && !ilOut ? outstr2 : nullptr, paired ? unpaired1 : nullptr,
                                      paired ? unpaired2 : nullptr, failed};
-    const size_t cap[FP_FQ_OUTS] = {n1 + n2 + (n1 / 8 + 1) * 40 + 64, n1 + 64, n2 + 64, both + 64, n2 + 64, both + (both / 6 + 2) * 24 + 64};
+    const size_t cap[FP_FQ_OUTS] = {n1 + n2 + (n1 / 8 + 1) * 40 + 64, (ilOut ? both : n1) + 64, side2 + 64, both + 64, side2 + 64,
+                                    both + (both / 6 + 2) * 24 + 64};
     uint8_t* outs[FP_FQ_OUTS]; int64_t caps[FP_FQ_OUTS], ob[FP_FQ_OUTS];
     for (int s = 0; s < FP_FQ_OUTS; s++) {
         if (want[s]) mTextOut[s].resize(cap[s]);

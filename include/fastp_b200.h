@@ -535,6 +535,32 @@ int  fp_fastq_process_host_outs(fp_ctx* ctx, const uint8_t* text1, int64_t nbyte
                                 int64_t out_bytes[FP_FQ_OUTS], int64_t* n_units, int64_t* consumed1, int64_t* consumed2,
                                 fp_fastq_info* info1, fp_fastq_info* info2);
 
+/* Interleaved pairs (--interleaved_in, --stdout): mates alternate in one text, read 1 then read 2 (FastqReaderPair::read with
+ * interleaved = true, src/fastqreader.cpp:452-460).  The pair stream ends at the first record either mate's reader rejects (ReadPair::eof,
+ * src/read.cpp:203-205): a rejected mate 2 also drops the good mate 1 before it, and a lone last record is dropped without a message.
+ * fp_fastq_decode_interleaved is fp_fastq_decode for such a chunk: record r goes to side (r & 1), row (r >> 1), rows / lengths / records per
+ * side (all DEVICE).  capacity and info->n_records count PAIRS; info->error_record is the first bad record's index among the chunk's
+ * records (mates counted one by one).  A chunk that is not final and ends with a lone mate 1 is consumed up to that record's name line;
+ * a final one drops it and is consumed whole.  Capacity cuts after record 2 * capacity.  Synchronous.
+ * fp_fastq_encode_interleaved writes the --stdout stream of a paired ctx (src/peprocessor.cpp:579-581, singleOutput): for every pair,
+ * read 1's record as fp_fastq_encode writes it on out1, then read 2's as it writes it on out2 -- byte for byte the two streams interleaved
+ * record by record.  Arguments as fp_fastq_encode_merge (side 2's text may be side 1's).  FP_E_INVAL on a single-end ctx and on a ctx that
+ * merges pairs (its stdout stream is the merged one: fp_fastq_encode_merge with FP_FQ_OUT_MERGED).  Synchronous.
+ * fp_fastq_set_interleaved switches the text path (fp_fastq_process_host, _merge, _outs); both default to 0:
+ *   in = 1   text1 holds both mates: pass text2 NULL and nbytes2 0; *consumed2 is 0 and *info2 is zeroed, info1 counts pairs.
+ *   out = 1  the FP_FQ_OUT_R1 buffer (out1) receives the interleaved stream; an FP_FQ_OUT_R2 buffer (out2) is refused.
+ * FP_E_INVAL, nothing changed: `in` on a single-end ctx, `out` on a single-end ctx or one that merges pairs.  The round loop itself refuses
+ * (FP_E_INVAL, nothing touched) text2 / nbytes2 with `in`, and an out2 buffer with `out`. */
+int  fp_fastq_decode_interleaved(fp_ctx* ctx, const uint8_t* d_text, int64_t nbytes, int32_t final_chunk, int32_t phred64,
+                                 uint8_t* d_seq1, uint8_t* d_qual1, uint16_t* d_len1, fp_fastq_rec* d_recs1,
+                                 uint8_t* d_seq2, uint8_t* d_qual2, uint16_t* d_len2, fp_fastq_rec* d_recs2,
+                                 int64_t capacity, fp_fastq_info* info);
+int  fp_fastq_encode_interleaved(fp_ctx* ctx, const uint8_t* d_text1, const fp_fastq_rec* d_recs1, const uint8_t* d_text2, const fp_fastq_rec* d_recs2,
+                                 const fp_read_result* d_res1, const fp_read_result* d_res2,
+                                 const uint8_t* d_seq1, const uint8_t* d_qual1, const uint8_t* d_seq2, const uint8_t* d_qual2,
+                                 int64_t n, uint8_t* d_out, int64_t out_cap, int64_t* out_bytes);
+int  fp_fastq_set_interleaved(fp_ctx* ctx, int32_t in, int32_t out);
+
 /* ---------------- duplication bloom filter (SURVEY.md 8(f) rank 2; src/duplicate.cpp) ----------------
  * fp_dup_check replaces Duplicate::checkRead / checkPair (src/duplicate.cpp:126-154) for a batch in DEVICE memory: d_is_dup[i]
  * (nullable) = what the reference returns for unit i when units are fed in index order, batch after batch -- deterministic, not
