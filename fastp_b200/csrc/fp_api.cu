@@ -348,6 +348,9 @@ static int ctx_init(fp_ctx* c, const fp_params* p, int device, int64_t max_batch
             const auto& cs = c->overrep[sd];
             fp_overrep_side& S = c->ovr_side[sd];
             S.K = (int)cs.size(); S.eval_len = sd ? p->seq_len2 : p->seq_len1;
+            /* a side without candidates has no table: bitmap_mask -1 makes the scan kernel's occupancy copy (words 0 .. mask >> 5)
+               empty for it, so the kernel never reads its null bitmap when the other mate has candidates */
+            S.bitmap_mask = -1;
             if (S.K == 0) continue;
             std::vector<uint8_t> blob; std::vector<int32_t> off, len;
             for (auto& q : cs) { off.push_back((int32_t)blob.size()); len.push_back((int32_t)q.size()); blob.insert(blob.end(), q.begin(), q.end()); }

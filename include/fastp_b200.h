@@ -107,7 +107,10 @@ typedef struct fp_params {
     /* sequence lengths from the pre-scan (Options::seqLen1/2, options.h:366-367): Stats::mEvaluatedSeqLen */
     int32_t seq_len1, seq_len2;
     /* OverrepresentedSequenceAnasysOptions options.h:71-80 + the candidate lists the Evaluator pre-scan produced
-     * (Options::overRepSeqs1/2, options.h:364-365; Evaluator::computeOverRepSeq evaluator.cpp:78-169 stays on the host) */
+     * (Options::overRepSeqs1/2, options.h:364-365; Evaluator::computeOverRepSeq evaluator.cpp:78-169 stays on the host).
+     * Domain, as the Evaluator produces it: seq_len1/2 >= 2 (the fifth scan length is min(150, seq_len - 2)); each list free of
+     * duplicates and of empty strings (the keys of a map), of any size, empty for one mate or both; reads may be longer or shorter
+     * than seq_len (hit positions at or past seq_len are not counted in the dist). */
     int32_t overrep_enabled;
     int32_t overrep_sampling;               /* default 20 */
     int32_t n_overrep1;

@@ -51,7 +51,55 @@ static inline int base2val(uint8_t b) {  /* stats.cpp:293-318 */
     switch (b) { case 'A': return 0; case 'T': return 1; case 'C': return 2; case 'G': return 3; default: return -1; }
 }
 
-static void stat_read(const fp_params* p, int64_t* C, const fp_counter_layout* L, int s, const uint8_t* seq, const uint8_t* qual, int len) {
+/* mOverRepSeq (stats.h:91) is a std::map<string, long>: its keys ordered by bytes, looked up in O(log K).  Restated as the candidates
+ * of each side sorted by (bytes, index); a window is found by binary search, the lowest index among equal strings wins (the lists
+ * are duplicate-free, as the map's keys are, so that tie never arises in practice). */
+typedef struct { const char* s; int len, k; } ovr_key;
+typedef struct { ovr_key* keys[2]; int K[2]; } ovr_index;
+
+static int ovr_key_cmp(const void* a, const void* b) {
+    const ovr_key *x = (const ovr_key*)a, *y = (const ovr_key*)b;
+    const int c = strcmp(x->s, y->s);
+    return c ? c : (x->k > y->k) - (x->k < y->k);
+}
+
+static int ovr_index_make(ovr_index* X, const fp_params* p, const fp_counter_layout* L) {
+    memset(X, 0, sizeof(*X));
+    if (!p->overrep_enabled) return 1;
+    for (int side = 0; side < 2; side++) {
+        const int K = L->n_overrep[side];
+        const char* const* cands = side ? p->overrep_seqs2 : p->overrep_seqs1;
+        if (K <= 0) continue;
+        X->keys[side] = (ovr_key*)malloc((size_t)K * sizeof(ovr_key));
+        if (!X->keys[side]) return 0;
+        for (int k = 0; k < K; k++) { X->keys[side][k].s = cands[k]; X->keys[side][k].len = (int)strlen(cands[k]); X->keys[side][k].k = k; }
+        qsort(X->keys[side], (size_t)K, sizeof(ovr_key), ovr_key_cmp);
+        X->K[side] = K;
+    }
+    return 1;
+}
+
+static void ovr_index_free(ovr_index* X) { free(X->keys[0]); free(X->keys[1]); }
+
+/* byte order of the window w[0, n) against key c (a shorter string that is a prefix of the other comes first) */
+static int ovr_window_cmp(const uint8_t* w, int n, const ovr_key* c) {
+    const int m = imin(n, c->len);
+    const int r = memcmp(w, c->s, (size_t)m);
+    return r ? r : (n > c->len) - (n < c->len);
+}
+
+/* mOverRepSeq.count(seq) > 0: index of the candidate equal to w[0, n), -1 if none */
+static int ovr_find(const ovr_index* X, int side, const uint8_t* w, int n) {
+    if (n < 0) return -1;                                              /* step 5 of seq_len < 2: outside the domain (fp_params) */
+    int lo = 0, hi = X->K[side];                                       /* lower bound of w in (bytes, index) order */
+    while (lo < hi) {
+        const int mid = lo + (hi - lo) / 2;
+        if (ovr_window_cmp(w, n, &X->keys[side][mid]) > 0) lo = mid + 1; else hi = mid;
+    }
+    return lo < X->K[side] && ovr_window_cmp(w, n, &X->keys[side][lo]) == 0 ? X->keys[side][lo].k : -1;
+}
+
+static void stat_read(const fp_params* p, const ovr_index* X, int64_t* C, const fp_counter_layout* L, int s, const uint8_t* seq, const uint8_t* qual, int len) {
     C[fp_off_length_sum(L, s)] += len;                                  /* stats.cpp:194 */
     int kmer = 0;
     int needFullCompute = 1;
@@ -96,15 +144,12 @@ static void stat_read(const fp_params* p, int64_t* C, const fp_counter_layout* L
     if (p->overrep_enabled) {
         if (C[fp_off_reads(L, s)] % p->overrep_sampling == 0) {
             const int side = s >> 1;
-            const int K = L->n_overrep[side], evalLen = L->overrep_len[side];
-            const char* const* cands = side ? p->overrep_seqs2 : p->overrep_seqs1;
+            const int evalLen = L->overrep_len[side];
             const int steps[5] = {10, 20, 40, 100, imin(150, evalLen - 2)};
             for (int s5 = 0; s5 < 5; s5++) {
                 const int step = steps[s5];
                 for (int i = 0; i < len - step; i++) {
-                    int hit = -1;                                       /* mOverRepSeq.count(seq) > 0 */
-                    for (int k = 0; k < K && hit < 0; k++)
-                        if ((int)strlen(cands[k]) == step && memcmp(cands[k], seq + i, (size_t)step) == 0) hit = k;
+                    const int hit = ovr_find(X, side, seq + i, step);  /* mOverRepSeq.count(seq) > 0 */
                     if (hit >= 0) {
                         C[fp_off_overrep_count(L, s, hit)]++;
                         for (int q = i; q < step + i && q < evalLen; q++) C[fp_off_overrep_dist(L, s, hit, q)]++;
@@ -575,10 +620,10 @@ static void fill_result(fp_read_result* o, const oread* r, const uint8_t* row, i
 /* ------------------------------------------------------------------------------------------
  * SingleEndProcessor::processSingleEnd loop body  src/seprocessor.cpp:204-296
  * ------------------------------------------------------------------------------------------ */
-static void process_se_one(const fp_params* p, const fp_counter_layout* L, int64_t* C,
+static void process_se_one(const fp_params* p, const ovr_index* X, const fp_counter_layout* L, int64_t* C,
                            uint8_t* seq, uint8_t* qual, int len, int dedupOut, fp_read_result* out) {
     int64_t* FR = C + L->off_filter;
-    stat_read(p, C, L, FP_STATS_PRE1, seq, qual, len);                     /* :211 */
+    stat_read(p, X, C, L, FP_STATS_PRE1, seq, qual, len);                     /* :211 */
     oread r = {seq, qual, len, 0};
     int frontTrimmed = 0, flags = dedupOut ? FP_F_DUPLICATE : 0, apos = 0, abases = 0, polyBase = 255, polyLen = 0;
     if (!trim_and_cut(p, &r, p->trim_front1, p->trim_tail1, &frontTrimmed)) r.is_null = 1;   /* :235 */
@@ -606,7 +651,7 @@ static void process_se_one(const fp_params* p, const fp_counter_layout* L, int64
     if (isAdapterDimer) { result = FP_FAIL_ADAPTER_DIMER; flags |= FP_F_ADAPTER_DIMER; }   /* :275-276 */
     FR[FP_FR_READSTATS + result] += 1;                                  /* :278 */
     if (!dedupOut && !r.is_null && result == FP_PASS_FILTER)            /* :280-286 */
-        stat_read(p, C, L, FP_STATS_POST1, r.seq, r.qual, r.len);
+        stat_read(p, X, C, L, FP_STATS_POST1, r.seq, r.qual, r.len);
     fill_result(out, &r, seq, result, result, flags, apos, abases, polyBase, polyLen);
 }
 
@@ -614,13 +659,13 @@ static void process_se_one(const fp_params* p, const fp_counter_layout* L, int64
  * PairEndProcessor::processPairEnd loop body  src/peprocessor.cpp:383-643 (incl. merging mode :519-560 and dedupOut :397-401;
  * no overlapped_out / index filter / UMI) + statInsertSize :710-723
  * ------------------------------------------------------------------------------------------ */
-static void process_pe_one(const fp_params* p, const fp_counter_layout* L, int64_t* C,
+static void process_pe_one(const fp_params* p, const ovr_index* X, const fp_counter_layout* L, int64_t* C,
                            uint8_t* seq1, uint8_t* qual1, int len1, uint8_t* seq2, uint8_t* qual2, int len2, int dedupOut,
                            fp_read_result* out1, fp_read_result* out2, fp_ov_result* ovOut) {
     int64_t* FR = C + L->off_filter;
     int64_t* ISZ = C + L->off_isize;
-    stat_read(p, C, L, FP_STATS_PRE1, seq1, qual1, len1);                  /* :393-394 */
-    stat_read(p, C, L, FP_STATS_PRE2, seq2, qual2, len2);
+    stat_read(p, X, C, L, FP_STATS_PRE1, seq1, qual1, len1);                  /* :393-394 */
+    stat_read(p, X, C, L, FP_STATS_PRE2, seq2, qual2, len2);
     oread r1 = {seq1, qual1, len1, 0}, r2 = {seq2, qual2, len2, 0};
     int ft1 = 0, ft2 = 0;
     int flags1 = dedupOut ? FP_F_DUPLICATE : 0, flags2 = flags1, apos1 = 0, apos2 = 0, ab1 = 0, ab2 = 0, pb1 = 255, pb2 = 255, pl1 = 0, pl2 = 0;
@@ -734,7 +779,7 @@ static void process_pe_one(const fp_params* p, const fp_counter_layout* L, int64
             const int result = pass_filter(p, &m);                      /* :526 */
             FR[FP_FR_READSTATS + result] += 2;                          /* :527 */
             if (result == FP_PASS_FILTER) {                             /* :528-534: dedupOut is not consulted for a merged read */
-                stat_read(p, C, L, FP_STATS_POST1, mseq, mqual, m.len);
+                stat_read(p, X, C, L, FP_STATS_POST1, mseq, mqual, m.len);
                 FR[FP_FR_MERGED_PAIRS] += 1;                            /* mergedCount -> addMergedPairs :694 */
             }
             result1 = result2 = pv = result;
@@ -748,9 +793,9 @@ static void process_pe_one(const fp_params* p, const fp_counter_layout* L, int64
                 flags1 |= FP_F_ADAPTER_DIMER; flags2 |= FP_F_ADAPTER_DIMER;
             }
             FR[FP_FR_READSTATS + result1] += 1;
-            if (result1 == FP_PASS_FILTER && !dedupOut) stat_read(p, C, L, FP_STATS_POST1, r1.seq, r1.qual, r1.len);   /* :547 */
+            if (result1 == FP_PASS_FILTER && !dedupOut) stat_read(p, X, C, L, FP_STATS_POST1, r1.seq, r1.qual, r1.len);   /* :547 */
             FR[FP_FR_READSTATS + result2] += 1;
-            if (result2 == FP_PASS_FILTER && !dedupOut) stat_read(p, C, L, FP_STATS_POST1, r2.seq, r2.qual, r2.len);   /* :553; read 2 into read 1's Stats: :555 */
+            if (result2 == FP_PASS_FILTER && !dedupOut) stat_read(p, X, C, L, FP_STATS_POST1, r2.seq, r2.qual, r2.len);   /* :553; read 2 into read 1's Stats: :555 */
             pv = imax(result1, result2);
             mergeProcessed = 1;
         }
@@ -765,8 +810,8 @@ static void process_pe_one(const fp_params* p, const fp_counter_layout* L, int64
         pv = imax(result1, result2);
         FR[FP_FR_READSTATS + pv] += 2;                                  /* :573 */
         if (!dedupOut && !p->merge_enabled && !r1.is_null && result1 == FP_PASS_FILTER && !r2.is_null && result2 == FP_PASS_FILTER) {   /* :575-591 */
-            stat_read(p, C, L, FP_STATS_POST1, r1.seq, r1.qual, r1.len);
-            stat_read(p, C, L, FP_STATS_POST2, r2.seq, r2.qual, r2.len);
+            stat_read(p, X, C, L, FP_STATS_POST1, r1.seq, r1.qual, r1.len);
+            stat_read(p, X, C, L, FP_STATS_POST2, r2.seq, r2.qual, r2.len);
         }
     }
     fill_result(out1, &r1, seq1, result1, pv, flags1, apos1, ab1, pb1, pl1);
@@ -779,17 +824,20 @@ int fp_oracle_process_dedup(const fp_params* p, const fp_counter_layout* L, cons
                             fp_read_result* out1, fp_read_result* out2, fp_ov_result* ov, int64_t* counters) {
     if (!p || !L || !b || !out1 || !counters) return FP_E_INVAL;
     if (b->stride > FP_MAX_STRIDE) return FP_E_INVAL;
+    if (p->paired && !out2) return FP_E_INVAL;
+    ovr_index X;
+    if (!ovr_index_make(&X, p, L)) { ovr_index_free(&X); return FP_E_NOMEM; }
     if (p->paired) {
-        if (!out2) return FP_E_INVAL;
         for (int64_t i = 0; i < b->n; i++)
-            process_pe_one(p, L, counters,
+            process_pe_one(p, &X, L, counters,
                            b->seq1 + i * b->stride, b->qual1 + i * b->stride, b->len1[i],
                            b->seq2 + i * b->stride, b->qual2 + i * b->stride, b->len2[i], is_dup && is_dup[i],
                            out1 + i, out2 + i, ov ? ov + i : NULL);
     } else {
         for (int64_t i = 0; i < b->n; i++)
-            process_se_one(p, L, counters, b->seq1 + i * b->stride, b->qual1 + i * b->stride, b->len1[i], is_dup && is_dup[i], out1 + i);
+            process_se_one(p, &X, L, counters, b->seq1 + i * b->stride, b->qual1 + i * b->stride, b->len1[i], is_dup && is_dup[i], out1 + i);
     }
+    ovr_index_free(&X);
     return FP_OK;
 }
 

@@ -81,10 +81,12 @@ def pack_rows(lib, b, arrs, paired, threads=4):
     return pb, keep
 
 
-def run_gpu(params, arrs, cycles, mode="device", ctx=None, splits=1, is_dup=None):
+def run_gpu(params, arrs, cycles, mode="device", ctx=None, splits=1, is_dup=None, bounds=None, first_index=None, indexed=None):
     """Run the CUDA hot path over a COPY of arrs; same return shape as fp_testlib.run_cpu.
     is_dup (mode "device" only): --dedup flags of the units, uploaded and given to every launch through fp_set_dup_flags at that
-    launch's first unit, and cleared afterwards."""
+    launch's first unit, and cleared afterwards.
+    bounds (mode "device"): the launches' unit boundaries [0, ..., n] instead of `splits` even ones.  first_index: launches carry
+    FP_B_INDEXED with first_read_index = first_index + their first unit -- all of them, or those whose number is in `indexed`."""
     torch = _torch()
     paired = bool(params.paired)
     n, stride = arrs["seq1"].shape
@@ -111,16 +113,18 @@ def run_gpu(params, arrs, cycles, mode="device", ctx=None, splits=1, is_dup=None
             flags = np.ascontiguousarray(is_dup, np.uint8)
             assert flags.shape == (n,)
             d_dup = torch.from_numpy(np.concatenate([flags, np.zeros(1, np.uint8)])).cuda()
-        bounds = [n * i // splits for i in range(splits + 1)]
-        for lo, hi in zip(bounds[:-1], bounds[1:]):          # consecutive sub-batches of one stream (counters accumulate)
+        bounds = bounds if bounds is not None else [n * i // splits for i in range(splits + 1)]
+        for launch, (lo, hi) in enumerate(zip(bounds[:-1], bounds[1:])):     # consecutive sub-batches of one stream (counters accumulate)
             if d_dup is not None:
                 capi.check(lib.fp_set_dup_flags(ctx.h, d_dup.data_ptr() + lo), lib)
             sb = capi.Batch()
             sb.n, sb.stride = hi - lo, stride
+            if first_index is not None and (indexed is None or launch in indexed):
+                sb.flags, sb.first_read_index = capi.FP_B_INDEXED, first_index + lo
             for k, v in t.items():
                 setattr(sb, k, v.data_ptr() + lo * (2 if k.startswith("len") else stride))
             if paired:
-                assert splits == 1 or not params.correction_enabled, "patch indices are batch-local"
+                assert len(bounds) == 2 or not params.correction_enabled, "patch indices are batch-local"
                 capi.check(lib.fp_process_pe(ctx.h, C.byref(sb), d_out1.data_ptr() + lo * 16, d_out2.data_ptr() + lo * 16, d_ov.data_ptr() + lo * 8,
                                              d_patch.data_ptr(), cap, d_np.data_ptr(), None), lib)
             else:
