@@ -192,6 +192,9 @@ SYMBOLS = {
                                     + [C.c_int64, C.POINTER(FastqInfo)]),
     "fp_fastq_encode_interleaved": (C.c_int, [C.c_void_p] + [C.c_void_p] * 10 + [C.c_int64, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]),
     "fp_fastq_set_interleaved": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
+    "fp_set_overlapped_sink": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "fp_fastq_encode_overlapped": (C.c_int, [C.c_void_p] + [C.c_void_p] * 7 + [C.c_int64, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]),
+    "fp_fastq_set_overlapped_out": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]),
 }
 
 

@@ -109,7 +109,8 @@ struct fp_ctx {
     /* FASTQ codec workspaces (grown on demand) and the buffers of fp_fastq_process_host */
     struct Buf { void* p = nullptr; size_t cap = 0; };
     Buf fq_term, fq_bcnt, fq_agg, fq_bstate, fq_brec, fq_recline, fq_recend, fq_info, fq_bsum;
-    Buf fqh_text[2], fqh_seq[2], fqh_qual[2], fqh_len[2], fqh_recs[2], fqh_res[2], fqh_ov, fqh_out[2], fqh_outbuf[2][6], fqh_recend[2];
+    Buf fqh_text[2], fqh_seq[2], fqh_qual[2], fqh_len[2], fqh_recs[2], fqh_res[2], fqh_ov, fqh_out[2], fqh_outbuf[2][FP_FQ_OUTS + 1], fqh_recend[2];
+    Buf fqh_ovx;                            /* the round's --overlapped_out analysis (fp_fastq_set_overlapped_out) */
     unsigned int *fq_hinfo = nullptr, *fq_hinfo_dev = nullptr;      /* mapped pinned control words */
     cudaStream_t fq_stream_out = nullptr;
     cudaEvent_t fq_ev_up = nullptr, fq_ev_out[2] = {nullptr, nullptr};
@@ -120,6 +121,9 @@ struct fp_ctx {
     unsigned long long* d_dup_count = nullptr;
     int64_t dup_total = 0;
     const uint8_t* dup_flags = nullptr;     /* fp_set_dup_flags: --dedup flags of the batch the next launch works on */
+    fp_overlapped_result* ovx = nullptr;    /* fp_set_overlapped_sink: --overlapped_out analysis of the next launch's units */
+    uint8_t* fq_ov_out = nullptr;           /* fp_fastq_set_overlapped_out: host output of the text path's --overlapped_out stream */
+    int64_t fq_ov_cap = 0, *fq_ov_bytes = nullptr;
     int fq_dup_level = 0, fq_dedup = 0;     /* fp_fastq_set_dedup */
     int fq_il_in = 0, fq_il_out = 0;        /* fp_fastq_set_interleaved */
     Buf fq_dupflags;
@@ -177,7 +181,8 @@ static size_t smem_layout_for_tile(fp_ctx* c, int T, fp_smem_layout& sl) {
     /* ---- tables that live for the whole kernel: sink, LUTs, histograms, delta accumulators, block counters ---- */
     size_t off = 0;
     sl.off_dummy = (int)off; off += 128;
-    sl.off_lut = (int)off; off += align_up((size_t)3 * (S + 2) * 2, 16);
+    /* PE: a fourth table, the zero diff limits of --overlapped_out; the 4 KB alignment below absorbs it at every PE stride */
+    sl.off_lut = (int)off; off += align_up((size_t)(sides == 2 ? 4 : 3) * (S + 2) * 2, 16);
     sl.off_delta = (int)off; off += (size_t)sides * (size_t)S * 20 * 4;      /* before the aligned tables: fills what the alignment would waste */
     /* the two histograms are addressed as (field | table address): the 5-mer tables (4 KB per side, counts then signed deltas) must
        start on a 4 KB boundary of the SHARED WINDOW (c->smem_base = window address of dynamic shared memory, probed at fp_ctx_create),
@@ -466,7 +471,7 @@ extern "C" void fp_ctx_destroy(fp_ctx* c) {
         fp_ctx::Buf* all[] = {&c->fq_term, &c->fq_bcnt, &c->fq_agg, &c->fq_bstate, &c->fq_brec, &c->fq_recline, &c->fq_recend, &c->fq_info, &c->fq_bsum,
                               &c->fqh_text[0], &c->fqh_text[1], &c->fqh_seq[0], &c->fqh_seq[1], &c->fqh_qual[0], &c->fqh_qual[1], &c->fqh_len[0], &c->fqh_len[1],
                               &c->fqh_recs[0], &c->fqh_recs[1], &c->fqh_res[0], &c->fqh_res[1], &c->fqh_ov, &c->fqh_out[0], &c->fqh_out[1],
-                              &c->fqh_recend[0], &c->fqh_recend[1], &c->fq_dupflags};
+                              &c->fqh_recend[0], &c->fqh_recend[1], &c->fq_dupflags, &c->fqh_ovx};
         for (auto& round : c->fqh_outbuf) for (auto& b : round) fq_free(b);
         if (c->dup.bits) cudaFree(c->dup.bits);
         cudaFree(c->d_dup_primes); cudaFree(c->d_dup_count);
@@ -553,6 +558,7 @@ static int launch_chain(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
     a.b = *b; a.out1 = out1; a.out2 = out2; a.ov = ov;
     a.sink.patches = patches; a.sink.cap = patches ? patch_cap : 0; a.sink.count = n_patches;
     a.is_dup = c->dup_flags;
+    a.ovx = c->p.paired ? c->ovx : nullptr;
     a.events.events = c->ev_dev; a.events.cap = c->ev_dev ? c->ev_cap : 0; a.events.count = c->ev_count;
     a.counters = reinterpret_cast<unsigned long long*>(c->d_raw);
     a.n_tiles = (b->n + c->tile - 1) / c->tile;
@@ -873,6 +879,7 @@ static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
     if (hp_n) *hp_n = 0;
     /* the chain indexes the flags by the unit's index in its LAUNCH, and a host batch is launched chunk by chunk */
     if (c->dup_flags) return set_err(FP_E_INVAL, "duplicate flags are set (fp_set_dup_flags): they belong to one fp_process_se / _pe launch, not to a host batch");
+    if (c->ovx) return set_err(FP_E_INVAL, "an overlapped sink is set (fp_set_overlapped_sink): it belongs to one fp_process_pe launch, not to a host batch");
     CK(cudaSetDevice(c->device));
     int rc = ensure_staging(c);
     if (rc) return rc;
@@ -1465,6 +1472,19 @@ extern "C" int fp_fastq_encode_merge(fp_ctx* c, int32_t which, const uint8_t* d_
     return fastq_encode_impl<FQ_SEL_MERGED>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
 }
 
+extern "C" int fp_fastq_encode_overlapped(fp_ctx* c, const uint8_t* d_text1, const fp_fastq_rec* d_recs1, const fp_read_result* d_res1,
+                                          const fp_read_result* d_res2, const fp_overlapped_result* d_ovx, const uint8_t* d_seq1, const uint8_t* d_qual1,
+                                          int64_t n, uint8_t* d_out, int64_t out_cap, int64_t* out_bytes) {
+    if (!c || !out_bytes) return set_err(FP_E_INVAL, "null argument");
+    *out_bytes = 0;
+    if (!c->p.paired) return set_err(FP_E_INVAL, "ctx was created for single-end data: --overlapped_out needs pairs");
+    if (n <= 0) return FP_OK;
+    if (!d_text1 || !d_recs1 || !d_res1 || !d_res2 || !d_ovx || !d_seq1 || !d_qual1 || (out_cap > 0 && !d_out)) return set_err(FP_E_INVAL, "null argument");
+    fq_merge_args M{};
+    M.res2 = d_res2; M.ovx = d_ovx;
+    return fastq_encode_impl<FQ_SEL_OVERLAPPED>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
+}
+
 /* the argument rules of fp_fastq_encode_rejects and fp_fastq_process_host_outs (options.cpp:136-143, :222-229) */
 static int fastq_rejects_check(const fp_ctx* c, int writers) {
     if (writers & ~(FP_FQ_W_UNPAIRED1 | FP_FQ_W_UNPAIRED2)) return set_err(FP_E_INVAL, "writers holds bits other than FP_FQ_W_UNPAIRED1 / FP_FQ_W_UNPAIRED2");
@@ -1501,17 +1521,25 @@ extern "C" int fp_fastq_encode_rejects(fp_ctx* c, int32_t which, int32_t writers
 
 /* The round loop of the text path.  outs / ocap / out_bytes are indexed by FP_FQ_OUT_*; a NULL buffer is not encoded.  merging: the ctx
    merges pairs, so every round also keeps the chain's overlap results for the merged stream.  The reject streams read the round's decoded
-   lengths (fqh_len, which the chain leaves as they are) and take the unpaired writers from which unpaired buffers are given. */
+   lengths (fqh_len, which the chain leaves as they are) and take the unpaired writers from which unpaired buffers are given.  The
+   --overlapped_out output of fp_fastq_set_overlapped_out is one more stream, index FP_FQ_OUTS: its rounds keep the chain's exact-overlap
+   analysis (fqh_ovx). */
 static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbytes1, const uint8_t* text2, int64_t nbytes2,
-                                   int32_t final_chunk, int32_t phred64, uint8_t* const outs[FP_FQ_OUTS], const int64_t ocap[FP_FQ_OUTS],
-                                   int64_t* const out_bytes[FP_FQ_OUTS],
+                                   int32_t final_chunk, int32_t phred64, uint8_t* const outs_in[FP_FQ_OUTS], const int64_t ocap_in[FP_FQ_OUTS],
+                                   int64_t* const out_bytes_in[FP_FQ_OUTS],
                                    int64_t* n_units, int64_t* consumed1, int64_t* consumed2, fp_fastq_info* info1, fp_fastq_info* info2) {
     const int sides = c->p.paired ? 2 : 1;
+    constexpr int NOUT = FP_FQ_OUTS + 1, OVX = FP_FQ_OUTS;
+    uint8_t* outs[NOUT]; int64_t ocap[NOUT]; int64_t* out_bytes[NOUT];
+    for (int s = 0; s < FP_FQ_OUTS; s++) { outs[s] = outs_in[s]; ocap[s] = ocap_in[s]; out_bytes[s] = out_bytes_in[s]; }
+    outs[OVX] = sides == 2 ? c->fq_ov_out : nullptr; ocap[OVX] = c->fq_ov_cap; out_bytes[OVX] = sides == 2 ? c->fq_ov_bytes : nullptr;
+    const bool ovx = outs[OVX] != nullptr;
     const bool merging = c->p.merge_enabled && sides == 2;
     const int writers = (outs[FP_FQ_OUT_UNPAIRED1] ? FP_FQ_W_UNPAIRED1 : 0) | (outs[FP_FQ_OUT_UNPAIRED2] ? FP_FQ_W_UNPAIRED2 : 0);
     /* fp_fastq_set_interleaved: mates alternate in text1 (one upload, one decode per round); out1 receives read 1 and read 2 of every pair */
     const bool il_in = c->fq_il_in && sides == 2, il_out = c->fq_il_out && sides == 2 && !merging;
     if (c->dup_flags) return set_err(FP_E_INVAL, "duplicate flags are set (fp_set_dup_flags): the text path runs its own duplicate filter (fp_fastq_set_dedup)");
+    if (c->ovx) return set_err(FP_E_INVAL, "an overlapped sink is set (fp_set_overlapped_sink): the text path keeps its own (fp_fastq_set_overlapped_out)");
     if (il_in && (text2 || nbytes2 != 0)) return set_err(FP_E_INVAL, "interleaved input: both mates are in text1 (pass text2 NULL and nbytes2 0)");
     if (il_out && outs[FP_FQ_OUT_R2]) return set_err(FP_E_INVAL, "interleaved output: both reads go to out1 (pass no out2 buffer)");
     CK(cudaSetDevice(c->device));
@@ -1540,7 +1568,8 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
         if ((rc = fq_ensure(c->fqh_res[s], (size_t)cap * sizeof(fp_read_result)))) return rc;
     }
     if (merging && (rc = fq_ensure(c->fqh_ov, (size_t)cap * sizeof(fp_ov_result)))) return rc;
-    int64_t upl[2] = {0, 0}, start[2] = {0, 0}, obytes[FP_FQ_OUTS] = {0}, units = 0;
+    if (ovx && (rc = fq_ensure(c->fqh_ovx, (size_t)cap * sizeof(fp_overlapped_result)))) return rc;
+    int64_t upl[2] = {0, 0}, start[2] = {0, 0}, obytes[NOUT] = {0}, units = 0;
     fp_fastq_info agg[2]; memset(agg, 0, sizeof(agg)); agg[0].error_record = agg[1].error_record = -1;
     int flip = 0;
     auto upload_more = [&]() -> int {
@@ -1608,6 +1637,8 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
             }
             struct FlagsBack { fp_ctx* c; const uint8_t* f; ~FlagsBack() { c->dup_flags = f; } } flags_back{c, saved_flags};
             if (sides == 2) {
+                c->ovx = ovx ? (fp_overlapped_result*)c->fqh_ovx.p : nullptr;   /* for this launch only (the sink was refused above) */
+                struct SinkBack { fp_ctx* c; ~SinkBack() { c->ovx = nullptr; } } sink_back{c};
                 rc = launch_chain(c, &b, (fp_read_result*)c->fqh_res[0].p, (fp_read_result*)c->fqh_res[1].p, merging ? (fp_ov_result*)c->fqh_ov.p : nullptr,
                                   nullptr, 0, nullptr, st);
             } else rc = launch_chain(c, &b, (fp_read_result*)c->fqh_res[0].p, nullptr, nullptr, nullptr, 0, nullptr, st);
@@ -1615,7 +1646,7 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
             CK(cudaEventSynchronize(c->fq_ev_out[flip]));        /* the output buffers of two rounds ago have gone down */
             const uint8_t* rtext[2] = {(const uint8_t*)c->fqh_text[0].p + rstart[0], sides == 2 ? (const uint8_t*)c->fqh_text[1].p + rstart[1] : nullptr};
             if (il_in) rtext[1] = rtext[0];                       /* both mates' records point into the one text */
-            for (int s = 0; s < FP_FQ_OUTS; s++) {
+            for (int s = 0; s < NOUT; s++) {
                 if (!outs[s]) continue;                           /* caller does not want this stream's text */
                 fp_ctx::Buf& ob = c->fqh_outbuf[flip][s];
                 const int64_t room = std::max<int64_t>(ocap[s] - obytes[s], 0);
@@ -1630,7 +1661,10 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
                 const uint8_t* qual[2] = {(const uint8_t*)c->fqh_qual[0].p, (const uint8_t*)c->fqh_qual[1].p};
                 for (int attempt = 0; attempt < 2; attempt++) {   /* names longer than the estimate: encode again into a buffer of the exact size */
                     if ((rc = fq_ensure(ob, (size_t)want + 64))) return rc;
-                    if (s >= FP_FQ_OUT_UNPAIRED1)
+                    if (s == OVX)
+                        rc = fp_fastq_encode_overlapped(c, rtext[0], recs[0], res[0], res[1], (const fp_overlapped_result*)c->fqh_ovx.p, seq[0], qual[0],
+                                                        n, (uint8_t*)ob.p, want, &total);
+                    else if (s >= FP_FQ_OUT_UNPAIRED1)
                         rc = fp_fastq_encode_rejects(c, s, writers, rtext[0], recs[0], rtext[1], recs[1], res[0], res[1], seq[0], qual[0],
                                                      (const uint16_t*)c->fqh_len[0].p, seq[1], qual[1], (const uint16_t*)c->fqh_len[1].p,
                                                      n, (uint8_t*)ob.p, want, &total);
@@ -1668,7 +1702,7 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
     agg[0].consumed = start[0]; agg[1].consumed = start[1];
     if (il_in) memset(&agg[1], 0, sizeof(agg[1]));
     *n_units = units; *consumed1 = start[0]; if (consumed2) *consumed2 = start[1];
-    for (int s = 0; s < FP_FQ_OUTS; s++) if (out_bytes[s]) *out_bytes[s] = obytes[s];
+    for (int s = 0; s < NOUT; s++) if (out_bytes[s]) *out_bytes[s] = obytes[s];
     if (info1) *info1 = agg[0];
     if (info2 && sides == 2) *info2 = agg[1];
     return FP_OK;
@@ -1772,6 +1806,21 @@ extern "C" int fp_dup_check(fp_ctx* c, const fp_batch* b, int32_t accuracy_level
 extern "C" int fp_set_dup_flags(fp_ctx* c, const uint8_t* d_is_dup) {
     if (!c) return set_err(FP_E_INVAL, "null argument");
     c->dup_flags = d_is_dup;
+    return FP_OK;
+}
+
+extern "C" int fp_set_overlapped_sink(fp_ctx* c, fp_overlapped_result* d_ovx) {
+    if (!c) return set_err(FP_E_INVAL, "null argument");
+    if (!c->p.paired) return set_err(FP_E_INVAL, "ctx was created for single-end data: --overlapped_out needs pairs");
+    c->ovx = d_ovx;
+    return FP_OK;
+}
+
+extern "C" int fp_fastq_set_overlapped_out(fp_ctx* c, uint8_t* buf, int64_t cap, int64_t* out_bytes) {
+    if (!c) return set_err(FP_E_INVAL, "null argument");
+    if (!c->p.paired) return set_err(FP_E_INVAL, "ctx was created for single-end data: --overlapped_out needs pairs");
+    if (buf && !out_bytes) return set_err(FP_E_INVAL, "null argument");
+    c->fq_ov_out = buf; c->fq_ov_cap = buf ? cap : 0; c->fq_ov_bytes = buf ? out_bytes : nullptr;
     return FP_OK;
 }
 

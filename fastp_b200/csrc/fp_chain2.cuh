@@ -1566,6 +1566,8 @@ __global__ void __launch_bounds__(kChainThreads, 1) fp_chain2_kernel(const fp_la
     for (int i = tid; i < SIDES * FP_QUAL_BINS; i += kChainThreads) D.qh[i] = 0;
     for (int i = tid; i < (int)(sizeof(BlockCounters) / 4); i += kChainThreads) reinterpret_cast<unsigned int*>(bc)[i] = 0;
     for (int i = tid; i < S + 2; i += kChainThreads) { s_lut[i] = c_p.lut_ovlimit[i]; s_lut[(S + 2) + i] = c_p.lut_lowq[i]; s_lut[2 * (S + 2) + i] = c_p.lut_mindiff[i]; }
+    if (PAIRED)                                   /* --overlapped_out's diff limits: min(overlapDiffLimit, overlap_len * 0) = 0 */
+        for (int i = tid; i < S + 2; i += kChainThreads) s_lut[3 * (S + 2) + i] = 0;
     if (tid == 0) { mbar_init(mbar, 1); s_qn[0] = 0; s_qn[1] = 0; s_qn[2] = 0; asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
     /* column-pass ownership: thread = (side, half-word column): cycles 2*hc, 2*hc+1 */
@@ -1954,6 +1956,16 @@ __global__ void __launch_bounds__(kChainThreads, 1) fp_chain2_kernel(const fp_la
                         if (t1) { if (lead) atomicAdd(&bc->fr[FP_FR_ADAPTER_READS], 1u); flags1 |= FP_F_ADAPTER_TRIMMED; }   /* :472-475 */
                         if (t2) { if (lead) atomicAdd(&bc->fr[FP_FR_ADAPTER_READS], 1u); flags2 |= FP_F_ADAPTER_TRIMMED; }
                         if ((t1 || t2) && r1.len <= c_p.dimer_max_len && r2.len <= c_p.dimer_max_len) dimer = true;   /* :480-484 */
+                    }
+                    if (a.ovx) {                                                                  /* --overlapped_out :488-495 */
+                        const int16_t* zlut = s_lut + 3 * (S + 2);                                /* analyze(..., diffPercentLimit 0) */
+                        fp_ov_result o; o.overlapped = 0; o.offset = 0; o.overlap_len = 0;
+                        if (both) o = (clean1 && clean2) ? t_analyze_planes(r1, r2, PW, zlut, sub, GL) : t_analyze_bytes(r1, r2, zlut);
+                        if (lead) {
+                            fp_overlapped_result ox; ox.overlapped = o.overlapped; ox._pad = 0; ox.offset = o.offset; ox.overlap_len = o.overlap_len;
+                            ox.r1_len = both ? (uint16_t)r1.len : 0;
+                            a.ovx[gi] = ox;
+                        }
                     }
                     if (both && c_p.polyx) {                                                      /* :506-509 */
                         const uint32_t px1 = t_polyx_cannot_trim(r1, PW, c_p.polyx_min) ? 0u : t_trim_polyx(r1.seq() + r1.front, r1.len, c_p.polyx_min);

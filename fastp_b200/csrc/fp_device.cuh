@@ -388,6 +388,7 @@ struct fp_launch_args {
     unsigned long long* counters;    /* global int64 block (two's complement adds) */
     long long n_tiles;
     fp_smem_layout sl;
+    fp_overlapped_result* ovx;       /* --overlapped_out (PE): the exact-overlap analysis of every unit (nullable) */
 };
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {

@@ -363,6 +363,8 @@ __global__ void fq_copy_u32_kernel(const unsigned int* src, unsigned int* dst) {
  *                  see fq_reject_plan
  *   FQ_SEL_INTERLEAVED  --stdout for pairs (peprocessor.cpp:579-581, singleOutput): for every unit, read 1's record as FQ_SEL_PLAIN writes
  *                  it on out1, then read 2's as it writes it on out2 -- out1 and out2 interleaved record by record
+ *   FQ_SEL_OVERLAPPED  --overlapped_out (peprocessor.cpp:488-495): one record per unit whose two reads trimAndCut kept and whose exact-overlap
+ *                  analysis (fq_merge_args.ovx) found an overlap; see fq_overlapped_window
  * The primary arrays (text, recs, res, seq, qual) are read 1's for FQ_SEL_MERGED and the reject streams, and the written side's for
  * FQ_SEL_SIDE; fq_merge_args carries the other side (FQ_SEL_SIDE reads only its records). */
 #define FQ_SCAN_ITEMS 2048
@@ -373,9 +375,11 @@ __global__ void fq_copy_u32_kernel(const unsigned int* src, unsigned int* dst) {
 #define FQ_SEL_UNPAIRED2 4
 #define FQ_SEL_FAILED 5
 #define FQ_SEL_INTERLEAVED 6
+#define FQ_SEL_OVERLAPPED 7
 struct fq_merge_args {
     const uint8_t* text2; const fq_rec* recs2; const fp_read_result* res2; const uint8_t* seq2; const uint8_t* qual2;
     const fp_ov_result* ov;
+    const fp_overlapped_result* ovx;      /* --overlapped_out only */
     int include_unmerged;
     /* reject streams only: decoded lengths of both sides (a dropped read is written whole), which unpaired writers exist
        (bit 0: --unpaired1, bit 1: a separate --unpaired2), whether the ctx merges; res2 == NULL for single-end */
@@ -515,9 +519,26 @@ __device__ __forceinline__ unsigned long long fq_write_reject(uint8_t* d, const 
     return fq_write_tagged(d, side ? M.text2 : text, side ? M.recs2[i] : recs[i], tag, (side ? M.seq2 : seq) + row, (side ? M.qual2 : qual) + row, n, lane);
 }
 
+/* ---- --overlapped_out ----
+ * The reference writes Read(r1 name, std::string(r1.seq.substr(max(0, offset)), overlap_len), r1 strand, the same of r1.qual): the
+ * constructor takes overlap_len as a start position, so the record holds read 1 after the overlap, [max(0, offset) + overlap_len, r1_len)
+ * of read 1 as the adapter trimmers left it.  That window starts at the record's front (polyX and max_len, which come later, only shorten
+ * read 1 from its 3' end, hence r1_len in the analysis result), and the row holds its corrected bases.  Returns whether the unit writes;
+ * its window is [from, from + n) of read 1's row (n may be 0). */
+__device__ __forceinline__ bool fq_overlapped_window(const fp_read_result& a, const fp_read_result& b, const fp_overlapped_result& ov, unsigned int& from, unsigned int& n) {
+    const unsigned int skip = (ov.offset > 0 ? (unsigned int)ov.offset : 0u) + (unsigned int)ov.overlap_len;
+    from = a.front + skip;
+    n = ov.r1_len > skip ? ov.r1_len - skip : 0u;
+    return ov.overlapped && !((a.flags | b.flags) & FP_F_DROPPED);
+}
+
 /* bytes unit i puts on the selected stream */
 template <int SEL>
 __device__ __forceinline__ unsigned long long fq_unit_size(const uint8_t* text, const fq_rec* recs, const fp_read_result* res, const fq_merge_args& M, long long i) {
+    if (SEL == FQ_SEL_OVERLAPPED) {
+        unsigned int from, n;
+        return fq_overlapped_window(res[i], M.res2[i], M.ovx[i], from, n) ? fq_tagged_size(recs[i], FQ_TAG_NONE, n) : 0ull;
+    }
     if (SEL == FQ_SEL_INTERLEAVED) {
         const fp_read_result a = res[i], b = M.res2[i];
         return (fq_written(a, a.pair_verdict) ? fq_record_size(recs[i], a) : 0ull) + (fq_written(b, b.pair_verdict) ? fq_record_size(M.recs2[i], b) : 0ull);
@@ -645,6 +666,13 @@ __global__ void __launch_bounds__(FQ_T) fq_encode_kernel(const uint8_t* text, co
                 }
                 const fp_read_result a = res[ri];
                 if (fq_written(a, a.pair_verdict)) fq_write_record(d, text, recs[ri], a, seq + row, qual + row, lane);
+                continue;
+            }
+            if (SEL == FQ_SEL_OVERLAPPED) {
+                unsigned int from, n;
+                fq_overlapped_window(res[ri], M.res2[ri], M.ovx[ri], from, n);
+                const size_t row = (size_t)ri * stride + from;
+                fq_write_tagged(d, text, recs[ri], FQ_TAG_NONE, seq + row, qual + row, n, lane);
                 continue;
             }
             if (SEL >= FQ_SEL_UNPAIRED1) {                             /* reject streams: the unit's records in plan order */

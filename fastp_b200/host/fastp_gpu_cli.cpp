@@ -26,7 +26,7 @@ static Read* readRecord(std::istream& in) {          /* FastqReader::read src/fa
 
 int main(int argc, char** argv) {
     Options opt;
-    std::string in1, in2, out1, out2, mergedOut, unpaired1, unpaired2, failedOut, json;
+    std::string in1, in2, out1, out2, mergedOut, unpaired1, unpaired2, failedOut, overlappedOut, json;
     int packSize = 1 << 16, maxLen = 0;
     bool deviceFastq = false, phred64 = false;
     bool interleavedIn = false, fromStdin = false, toStdout = false;     /* src/main.cpp:194-196 */
@@ -40,6 +40,7 @@ int main(int argc, char** argv) {
         else if (a == "-o" || a == "--out1") out1 = next(); else if (a == "-O" || a == "--out2") out2 = next();
         else if (a == "--unpaired1") unpaired1 = next(); else if (a == "--unpaired2") unpaired2 = next();
         else if (a == "--failed_out") failedOut = next();
+        else if (a == "--overlapped_out") overlappedOut = next();
         else if (a == "-j" || a == "--json") json = next();
         else if (a == "-A" || a == "--disable_adapter_trimming") opt.adapter.enabled = false;
         else if (a == "-a" || a == "--adapter_sequence") { opt.adapter.sequence = next(); opt.adapter.hasSeqR1 = true; }
@@ -76,7 +77,7 @@ int main(int argc, char** argv) {
         else { fprintf(stderr, "unknown flag %s\n", a.c_str()); return 2; }
     }
     if (in1.empty() && fromStdin && in2.empty()) in1 = "/dev/stdin";    /* src/options.cpp:85-93 */
-    if (in1.empty()) { fprintf(stderr, "usage: fastp_gpu_cli -i R1.fq [-I R2.fq] [--interleaved_in] [--stdin] [--stdout] [-o out1.fq] [-O out2.fq] [-m --merged_out merged.fq] [--unpaired1 u1.fq] [--unpaired2 u2.fq] [--failed_out failed.fq] [-j summary.json] [fastp flags]\n"); return 2; }
+    if (in1.empty()) { fprintf(stderr, "usage: fastp_gpu_cli -i R1.fq [-I R2.fq] [--interleaved_in] [--stdin] [--stdout] [-o out1.fq] [-O out2.fq] [-m --merged_out merged.fq] [--unpaired1 u1.fq] [--unpaired2 u2.fq] [--failed_out failed.fq] [--overlapped_out ov.fq] [-j summary.json] [fastp flags]\n"); return 2; }
     if (!deviceFastq && (interleavedIn || fromStdin || toStdout)) { fprintf(stderr, "ERROR: --interleaved_in / --stdin / --stdout need --device_fastq\n"); return 2; }
     const bool stdinInput = in1 == "/dev/stdin";         /* read as it comes: nothing may open it twice */
     if (toStdout) {                                      /* src/options.cpp:101-110 */
@@ -87,6 +88,7 @@ int main(int argc, char** argv) {
     if (!deviceFastq && !(unpaired1.empty() && unpaired2.empty() && failedOut.empty())) {
         fprintf(stderr, "ERROR: --unpaired1 / --unpaired2 / --failed_out need --device_fastq\n"); return 2;
     }
+    if (!deviceFastq && !overlappedOut.empty()) { fprintf(stderr, "ERROR: --overlapped_out needs --device_fastq\n"); return 2; }
     if (unpaired2.empty()) unpaired2 = unpaired1;       /* src/main.cpp:188-189 */
     auto fail = [](const char* msg) { fprintf(stderr, "ERROR: %s\n", msg); return 2; };
     if (opt.merge.enabled) {                            /* src/options.cpp:112-157 */
@@ -120,6 +122,7 @@ int main(int argc, char** argv) {
     if (!opt.paired) {                                  /* src/options.cpp:222-229 */
         if (!unpaired1.empty()) { std::cerr << "Not paired-end mode. Ignoring argument --unpaired1 = " << unpaired1 << std::endl; unpaired1.clear(); }
         if (!unpaired2.empty()) { std::cerr << "Not paired-end mode. Ignoring argument --unpaired2 = " << unpaired2 << std::endl; unpaired2.clear(); }
+        if (!overlappedOut.empty()) { std::cerr << "Not paired-end mode. Ignoring argument --overlapped_out = " << overlappedOut << std::endl; overlappedOut.clear(); }   /* :230-233 */
     }
     if (!unpaired1.empty()) {                           /* src/options.cpp:240-276 */
         if (unpaired1 == out1) return fail("--unpaired1 and --out1 shouldn't have same file name");
@@ -173,13 +176,14 @@ int main(int argc, char** argv) {
     if (chunkBytes == 0) chunkBytes = (size_t)packSize * (size_t)(2 * maxLen + 64);
     GpuChainWorker worker(&opt, maxLen, 0, packSize);
     if (!worker.ok()) { fprintf(stderr, "fastp_gpu_cli: %s\n", worker.error().c_str()); return 1; }
-    std::ofstream o1, o2, om, ou1, ou2, of;
+    std::ofstream o1, o2, om, ou1, ou2, of, oov;
     if (!out1.empty()) o1.open(out1);
     if (!out2.empty()) o2.open(out2);
     if (opt.merge.enabled && !mergedOut.empty()) om.open(mergedOut);
     if (unpairedLeft) ou1.open(unpaired1);              /* every writer creates its file, even one that stays empty */
     if (unpairedRight) ou2.open(unpaired2);
     if (!failedOut.empty()) of.open(failedOut);
+    if (!overlappedOut.empty()) oov.open(overlappedOut);  /* no file-name checks: the reference has none for it */
     if (deviceFastq) {
         if (opt.paired && (interleavedIn || (toStdout && !opt.merge.enabled)) && !worker.setInterleaved(interleavedIn, toStdout && !opt.merge.enabled)) {
             fprintf(stderr, "fastp_gpu_cli: interleaved text: %s\n", fp_last_error()); return 1;
@@ -202,7 +206,7 @@ int main(int argc, char** argv) {
         };
         auto gz_name = [](const std::string& n) { return n.size() > 3 && n.compare(n.size() - 3, 3, ".gz") == 0; };
         const bool zout1 = gz_name(out1), zout2 = gz_name(out2), zoutm = gz_name(mergedOut);
-        const bool zu1 = gz_name(unpaired1), zu2 = gz_name(unpaired2), zf = gz_name(failedOut);
+        const bool zu1 = gz_name(unpaired1), zu2 = gz_name(unpaired2), zf = gz_name(failedOut), zov = gz_name(overlappedOut);
         std::vector<uint8_t> zbuf;
         auto emit = [&](std::ofstream& o, const std::string& t, bool z) {
             if (!o.is_open() || t.empty()) return;
@@ -222,9 +226,10 @@ int main(int argc, char** argv) {
             fill(g1, buf1, eof1);
             if (twoFiles) fill(g2, buf2, eof2);
             const bool final = eof1 && eof2;
-            std::string s1, s2, sm, su1, su2, sf; size_t c1 = 0, c2 = 0; long units = 0;
+            std::string s1, s2, sm, su1, su2, sf, sov; size_t c1 = 0, c2 = 0; long units = 0;
             if (!worker.processFastqText(buf1.data(), buf1.size(), buf2.data(), buf2.size(), final, phred64, &s1, &s2, &c1, &c2, &units, &sm,
-                                         unpairedLeft ? &su1 : nullptr, unpairedRight ? &su2 : nullptr, failedOut.empty() ? nullptr : &sf)) {
+                                         unpairedLeft ? &su1 : nullptr, unpairedRight ? &su2 : nullptr, failedOut.empty() ? nullptr : &sf,
+                                         overlappedOut.empty() ? nullptr : &sov)) {
                 fprintf(stderr, "fastp_gpu_cli: %s\n", worker.error().c_str()); return 1;
             }
             if (toStdout) to_stdout(opt.merge.enabled ? (mergedOut.empty() ? sm : std::string()) : s1);    /* :672-678 */
@@ -234,6 +239,7 @@ int main(int argc, char** argv) {
             emit(ou1, su1, zu1);
             if (unpairedLeft) emit(ou2, su2, zu2);         /* the unpaired-2 text reaches its file only when both writers exist (peprocessor.cpp:681-686) */
             emit(of, sf, zf);
+            emit(oov, sov, zov);
             buf1.erase(0, c1); if (twoFiles) buf2.erase(0, c2);
             if (worker.inputEnded()) break;                    /* a reader gave up on a record: the reference stops reading there */
             if (final && (units == 0 || (buf1.empty() && buf2.empty()))) break;

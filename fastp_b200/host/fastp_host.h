@@ -99,7 +99,8 @@ public:
      * of pairs that did not merge; src/peprocessor.cpp:519-560) and outstr1 / outstr2 only the pairs that took neither branch.
      * `unpaired1` / `unpaired2` / `failed` receive --unpaired1 / --unpaired2 / --failed_out (src/seprocessor.cpp:280-290,
      * src/peprocessor.cpp:594-620); NULL means that writer does not exist, which decides where a pair with one failing read goes
-     * (fp_fastq_process_host_outs).  The unpaired ones are for paired runs without --include_unmerged. */
+     * (fp_fastq_process_host_outs).  The unpaired ones are for paired runs without --include_unmerged.  `overlapped` receives
+     * --overlapped_out (src/peprocessor.cpp:488-495, paired runs; fp_fastq_set_overlapped_out). */
     /* true once a reader rejected a record (strand line not '+', |quality| != |sequence|): like FastqReader::read returning NULL the
      * input ENDS there -- the caller stops feeding chunks (src/fastqreader.cpp:349-364) */
     bool inputEnded() const { return mInputEnded; }
@@ -115,7 +116,7 @@ public:
     bool processFastqText(const char* text1, size_t n1, const char* text2, size_t n2, bool final, bool phred64,
                           std::string* outstr1, std::string* outstr2, size_t* consumed1, size_t* consumed2, long* units,
                           std::string* merged = nullptr, std::string* unpaired1 = nullptr, std::string* unpaired2 = nullptr,
-                          std::string* failed = nullptr);
+                          std::string* failed = nullptr, std::string* overlapped = nullptr);
 
     /* end of run: what Stats::merge / FilterResult::merge hand to the reporters (src/peprocessor.cpp:217-234) */
     bool finish(Stats* pre1, Stats* post1, Stats* pre2, Stats* post2, FilterResult* fr, std::vector<long>* insertSizeHist);
@@ -133,7 +134,7 @@ private:
     uint16_t* mLen[2] = {nullptr, nullptr};
     fp_read_result* mRes[2] = {nullptr, nullptr};
     fp_ov_result* mOv = nullptr;
-    std::vector<uint8_t> mTextOut[FP_FQ_OUTS];      /* indexed by FP_FQ_OUT_*: merged, out1, out2, unpaired1, unpaired2, failed */
+    std::vector<uint8_t> mTextOut[FP_FQ_OUTS + 1];  /* indexed by FP_FQ_OUT_*: merged, out1, out2, unpaired1, unpaired2, failed; then overlapped */
     bool mInputEnded = false;
     bool mIlIn = false, mIlOut = false;
     std::string mError;

@@ -175,7 +175,8 @@ bool GpuChainWorker::processPairEnd(ReadPack* leftPack, ReadPack* rightPack, std
 
 bool GpuChainWorker::processFastqText(const char* text1, size_t n1, const char* text2, size_t n2, bool final, bool phred64,
                                       std::string* outstr1, std::string* outstr2, size_t* consumed1, size_t* consumed2, long* units,
-                                      std::string* merged, std::string* unpaired1, std::string* unpaired2, std::string* failed) {
+                                      std::string* merged, std::string* unpaired1, std::string* unpaired2, std::string* failed,
+                                      std::string* overlapped) {
     const bool paired = mParams.paired != 0, merging = paired && mParams.merge_enabled;
     const bool ilIn = paired && mIlIn, ilOut = paired && mIlOut;
     if (ilIn) n2 = 0;                                           /* both mates are in text1 */
@@ -197,9 +198,17 @@ bool GpuChainWorker::processFastqText(const char* text1, size_t n1, const char* 
         outs[s] = want[s] ? mTextOut[s].data() : nullptr;
         caps[s] = want[s] ? (int64_t)cap[s] : 0;
     }
+    /* --overlapped_out: at most one record of read 1 per pair, never longer than read 1's input record */
+    int64_t obOv = 0;
+    if (paired && overlapped) {
+        mTextOut[FP_FQ_OUTS].resize(n1 + 64);
+        if (fp_fastq_set_overlapped_out(mCtx, mTextOut[FP_FQ_OUTS].data(), (int64_t)(n1 + 64), &obOv) != FP_OK) { mError = fp_last_error(); return false; }
+    }
     const int rc = fp_fastq_process_host_outs(mCtx, t1, (int64_t)n1, t2, paired ? (int64_t)n2 : 0, final ? 1 : 0, phred64 ? 1 : 0, outs, caps, ob,
                                               &nu, &c1, paired ? &c2 : nullptr, &i1, paired ? &i2 : nullptr);
+    if (paired && overlapped) fp_fastq_set_overlapped_out(mCtx, nullptr, 0, nullptr);
     if (rc != FP_OK) { mError = fp_last_error(); return false; }
+    if (paired && overlapped) overlapped->append(reinterpret_cast<const char*>(mTextOut[FP_FQ_OUTS].data()), (size_t)obOv);
     if (i1.error == FP_FQ_ERR_STRIDE || (paired && i2.error == FP_FQ_ERR_STRIDE)) { mError = "a read is longer than the row stride (raise --max_read_len)"; return false; }
     if (i1.error != FP_FQ_OK || (paired && i2.error != FP_FQ_OK)) {
         const fp_fastq_info& bad = i1.error != FP_FQ_OK ? i1 : i2;

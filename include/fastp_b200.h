@@ -183,6 +183,13 @@ typedef struct fp_ov_result {
     int16_t offset, overlap_len, diff;
 } fp_ov_result;            /* 8 bytes */
 
+/* --overlapped_out: the overlap analysis of src/peprocessor.cpp:488-495 for one pair, and read 1's length when it ran (fp_set_overlapped_sink) */
+typedef struct fp_overlapped_result {
+    uint8_t  overlapped, _pad;
+    int16_t  offset, overlap_len;
+    uint16_t r1_len;       /* read 1's window length after the adapter trimmers (trimmed coordinates) */
+} fp_overlapped_result;    /* 8 bytes */
+
 /* --merge: the two pieces of a merged read (OverlapAnalysis::merge, overlapanalysis.cpp:149-157): merged = r1[0, len1) followed by the
  * reverse complement of r2[0, len2), both in TRIMMED coordinates (add fp_read_result.front for the row index); r2_len = out2.len. */
 static inline void fp_merged_lens(const fp_ov_result* ov, int r2_len, int* len1, int* len2) {
@@ -586,6 +593,30 @@ int  fp_dup_reset(fp_ctx* ctx);
  * `accuracy_level` on every round's decoded rows before the chain (0 = off) and drops duplicates from the output when `dedup` is set. */
 int  fp_set_dup_flags(fp_ctx* ctx, const uint8_t* d_is_dup);
 int  fp_fastq_set_dedup(fp_ctx* ctx, int32_t accuracy_level, int32_t dedup);
+
+/* --overlapped_out (src/peprocessor.cpp:488-495): after the adapter trimmers and before polyX, the reference runs the overlap analysis once
+ * more with diffPercentLimit 0 on every pair whose two reads trimAndCut kept -- whatever the filters, the dimer check, --dedup or merging
+ * later decide -- and, if it finds an overlap, writes a record with read 1's name and strand lines.  Its sequence is
+ * std::string(r1.substr(max(0, offset)), overlap_len): the two-argument constructor takes overlap_len as a START position, so the record
+ * holds read 1's (corrected) bases and qualities AFTER the overlap, r1[max(0, offset) + overlap_len, r1_len) in trimmed coordinates --
+ * empty whenever the overlap reaches the end of read 1.  r1_len is read 1's length at that point, before polyX and -b shorten it.
+ * The limit is min(overlapDiffLimit, 0) = 0, but like every no-gap analysis it is checked on the first min(overlap_len, 50) bases only: a
+ * longer overlap with mismatches further on is accepted.  --allow_gap_overlap_trimming does not apply.
+ * fp_set_overlapped_sink: `d_ovx` = DEVICE array that the next fp_process_pe launches fill, d_ovx[i] for unit i of the LAUNCH (overlapped = 0
+ * where trimAndCut dropped a read); NULL switches it off.  Same contract as fp_set_dup_flags: the pointer stays set until changed, and while
+ * it is set the host entry points (fp_process_*_host, _host_patches, _host_packed, fp_fastq_process_host*) return FP_E_INVAL and touch
+ * nothing.  FP_E_INVAL on a single-end ctx (the reference ignores the option there, src/options.cpp:230-233).
+ * fp_fastq_encode_overlapped writes the --overlapped_out text of a batch the chain worked on with the sink set (all pointers DEVICE): read 1's
+ * chunk and records, both reads' records (FP_F_DROPPED decides), d_ovx, read 1's rows as the chain left them; n, d_out, out_cap, out_bytes
+ * as fp_fastq_encode.  FP_E_INVAL on a single-end ctx.  Synchronous.
+ * fp_fastq_set_overlapped_out attaches a HOST output of `cap` bytes to the text path (fp_fastq_process_host, _merge, _outs): every round
+ * keeps the analysis and appends its records; *out_bytes is set by each call, FP_E_TOOLARGE as for the other streams.  buf NULL detaches it.
+ * FP_E_INVAL on a single-end ctx. */
+int  fp_set_overlapped_sink(fp_ctx* ctx, fp_overlapped_result* d_ovx);
+int  fp_fastq_encode_overlapped(fp_ctx* ctx, const uint8_t* d_text1, const fp_fastq_rec* d_recs1, const fp_read_result* d_res1,
+                                const fp_read_result* d_res2, const fp_overlapped_result* d_ovx, const uint8_t* d_seq1, const uint8_t* d_qual1,
+                                int64_t n, uint8_t* d_out, int64_t out_cap, int64_t* out_bytes);
+int  fp_fastq_set_overlapped_out(fp_ctx* ctx, uint8_t* buf, int64_t cap, int64_t* out_bytes);
 
 /* Host-side pre-scan (control plane, once per input, like the reference's Evaluator): the over-representation candidate list
  * Evaluator::computeOverRepSeq (src/evaluator.cpp:78-169) derives from the first 1.51 M bases of one input, here given as rows
