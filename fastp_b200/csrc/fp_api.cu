@@ -42,6 +42,40 @@ extern "C" int fp_version(void) { return 100; }
 
 struct EvPair { cudaEvent_t a, b; };
 
+/* memory a ctx owns, on the device (cudaMalloc) or pinned on the host (cudaMallocHost): freed with the ctx, grown by grow(); cap in bytes */
+template <class T, bool Pinned> struct Mem {
+    T* p = nullptr;
+    size_t cap = 0;
+    Mem() = default;
+    Mem(const Mem&) = delete;
+    Mem& operator=(const Mem&) = delete;
+    ~Mem() { release(); }
+    void release() {
+        if (p) { if (Pinned) cudaFreeHost(p); else cudaFree(p); }
+        p = nullptr; cap = 0;
+    }
+};
+template <class T> using DevBuf = Mem<T, false>;
+template <class T> using HostBuf = Mem<T, true>;
+
+/* at least `need` bytes (need + slack allocated when it grows).  The old buffer is gone before the new one is asked for, and the
+   pointer and capacity are recorded only once the allocation succeeded: after a failure b is empty and the next call allocates again */
+template <class T, bool Pinned> static cudaError_t grow(Mem<T, Pinned>& b, size_t need, size_t slack = 0) {
+    if (need <= b.cap) return cudaSuccess;
+    b.release();
+    void* q = nullptr;
+    const cudaError_t e = Pinned ? cudaMallocHost(&q, need + slack) : cudaMalloc(&q, need + slack);
+    if (e == cudaSuccess) { b.p = (T*)q; b.cap = need + slack; }
+    return e;
+}
+
+/* grow() for a buffer of the host pipeline, which work queued on either chunk stream may still be using: the device is idle first */
+template <class T, bool Pinned> static cudaError_t grow_idle(Mem<T, Pinned>& b, size_t need, size_t slack = 0) {
+    if (need <= b.cap) return cudaSuccess;
+    const cudaError_t e = cudaDeviceSynchronize();
+    return e != cudaSuccess ? e : grow(b, need, slack);
+}
+
 struct fp_ctx {
     int device = 0;
     fp_params p{};
@@ -79,8 +113,8 @@ struct fp_ctx {
     /* adapter-string events (fp_adapter_event) */
     fp_adapter_event* ev_dev = nullptr; uint32_t ev_cap = 0; uint32_t* ev_count = nullptr;      /* device sink (caller's memory) */
     fp_adapter_event* ev_host = nullptr; uint64_t ev_host_cap = 0; uint64_t* ev_host_n = nullptr;  /* host sink of the *_host entry points */
-    fp_adapter_event* d_ev[2] = {nullptr, nullptr}; uint32_t* d_nev[2] = {nullptr, nullptr};        /* per chunk slot */
-    fp_adapter_event* h_ev[2] = {nullptr, nullptr}; uint32_t* h_nev[2] = {nullptr, nullptr};
+    DevBuf<fp_adapter_event> d_ev[2]; DevBuf<uint32_t> d_nev[2];        /* per chunk slot */
+    HostBuf<fp_adapter_event> h_ev[2]; HostBuf<uint32_t> h_nev[2];
     uint32_t ev_chunk_cap = 0;
     int ovr_defer_post = 0;             /* fp_overrep_defer_post: the caller runs fp_overrep_post itself (sharded runs) */
     unsigned long long* d_pass_count = nullptr;
@@ -88,28 +122,26 @@ struct fp_ctx {
     long long *d_raw = nullptr, *d_fin = nullptr;
     /* host-mode staging (allocated lazily) */
     int64_t chunk = 0;
-    uint8_t* d_stage[2][4] = {{nullptr}};      /* seq1 qual1 seq2 qual2 */
-    uint16_t* d_stage_len[2][2] = {{nullptr}};
-    fp_read_result* d_out[2][2] = {{nullptr}};
-    fp_ov_result* d_ov[2] = {nullptr, nullptr};
-    fp_patch* d_patch[2] = {nullptr, nullptr};
-    unsigned int* d_npatch[2] = {nullptr, nullptr};
-    fp_patch* h_patch[4] = {nullptr, nullptr, nullptr, nullptr};      /* host side: 4 rotating buffers (chunk % 4), see process_host */
-    unsigned int* h_npatch[4] = {nullptr, nullptr, nullptr, nullptr};
+    DevBuf<uint8_t> d_stage[2][4];              /* seq1 qual1 seq2 qual2 */
+    DevBuf<uint16_t> d_stage_len[2][2];
+    DevBuf<fp_read_result> d_out[2][2];
+    DevBuf<fp_ov_result> d_ov[2];
+    DevBuf<fp_patch> d_patch[2];
+    DevBuf<unsigned int> d_npatch[2];
+    HostBuf<fp_patch> h_patch[4];               /* host side: 4 rotating buffers (chunk % 4), see process_host */
+    HostBuf<unsigned int> h_npatch[4];
     uint32_t patch_cap = 0;
-    uint8_t* d_pk[2][4] = {{nullptr}};          /* packed staging per chunk slot: bases1 qual1 bases2 qual2 */
-    fp_npos* d_npos[2] = {nullptr, nullptr};
-    size_t pk_cap_b = 0, pk_cap_q = 0, npos_cap = 0;
+    DevBuf<uint8_t> d_pk[2][4];                 /* packed or tight-pitch staging per chunk slot: bases1 qual1 bases2 qual2 */
+    DevBuf<fp_npos> d_npos[2];
     /* FP_B_PACK2BIT: pinned host staging of the packing team (4 slots so that it runs two chunks ahead of the copies) */
-    uint8_t* h_pkb[4][2] = {{nullptr}};
-    fp_npos* h_np[4] = {nullptr, nullptr, nullptr, nullptr};
-    size_t h_pkb_cap = 0, h_np_cap = 0;
+    HostBuf<uint8_t> h_pkb[4][2];
+    HostBuf<fp_npos> h_np[4];
     int host_threads = 0;                       /* 0 = default_host_threads() */
     cudaEvent_t chunk_done[4] = {nullptr, nullptr, nullptr, nullptr};   /* end of host chunk k's work on its stream, by k % 4 (cudaEventBlockingSync) */
     /* FASTQ codec workspaces (grown on demand) and the buffers of fp_fastq_process_host */
-    struct Buf { void* p = nullptr; size_t cap = 0; };
+    using Buf = DevBuf<void>;
     Buf fq_term, fq_bcnt, fq_agg, fq_bstate, fq_brec, fq_recline, fq_recend, fq_info, fq_bsum;
-    Buf fqh_text[2], fqh_seq[2], fqh_qual[2], fqh_len[2], fqh_recs[2], fqh_res[2], fqh_ov, fqh_out[2], fqh_outbuf[2][FP_FQ_OUTS + 1], fqh_recend[2];
+    Buf fqh_text[2], fqh_seq[2], fqh_qual[2], fqh_len[2], fqh_recs[2], fqh_res[2], fqh_ov, fqh_outbuf[2][FP_FQ_OUTS + 1], fqh_recend[2];
     Buf fqh_ovx;                            /* the round's --overlapped_out analysis (fp_fastq_set_overlapped_out) */
     unsigned int *fq_hinfo = nullptr, *fq_hinfo_dev = nullptr;      /* mapped pinned control words */
     cudaStream_t fq_stream_out = nullptr;
@@ -433,32 +465,6 @@ static int ctx_init(fp_ctx* c, const fp_params* p, int device, int64_t max_batch
     return FP_OK;
 }
 
-static void fq_free(fp_ctx::Buf& b) { if (b.p) cudaFree(b.p); b.p = nullptr; b.cap = 0; }
-
-static void free_staging(fp_ctx* c) {
-    for (int i = 0; i < 2; i++) {
-        for (int k = 0; k < 4; k++) { cudaFree(c->d_stage[i][k]); c->d_stage[i][k] = nullptr; }
-        for (int k = 0; k < 2; k++) { cudaFree(c->d_stage_len[i][k]); c->d_stage_len[i][k] = nullptr; cudaFree(c->d_out[i][k]); c->d_out[i][k] = nullptr; }
-        cudaFree(c->d_ov[i]); c->d_ov[i] = nullptr;
-        cudaFree(c->d_patch[i]); c->d_patch[i] = nullptr;
-        cudaFree(c->d_npatch[i]); c->d_npatch[i] = nullptr;
-        for (int k = 0; k < 4; k++) { cudaFree(c->d_pk[i][k]); c->d_pk[i][k] = nullptr; }
-        cudaFree(c->d_npos[i]); c->d_npos[i] = nullptr;
-        cudaFree(c->d_ev[i]); c->d_ev[i] = nullptr; cudaFree(c->d_nev[i]); c->d_nev[i] = nullptr;
-        if (c->h_ev[i]) cudaFreeHost(c->h_ev[i]); c->h_ev[i] = nullptr;
-        if (c->h_nev[i]) cudaFreeHost(c->h_nev[i]); c->h_nev[i] = nullptr;
-    }
-    for (int i = 0; i < 4; i++) {
-        if (c->h_patch[i]) cudaFreeHost(c->h_patch[i]); c->h_patch[i] = nullptr;
-        if (c->h_npatch[i]) cudaFreeHost(c->h_npatch[i]); c->h_npatch[i] = nullptr;
-        for (int k = 0; k < 2; k++) { if (c->h_pkb[i][k]) cudaFreeHost(c->h_pkb[i][k]); c->h_pkb[i][k] = nullptr; }
-        if (c->h_np[i]) cudaFreeHost(c->h_np[i]);
-        c->h_np[i] = nullptr;
-    }
-    c->h_pkb_cap = c->h_np_cap = 0;
-    c->chunk = 0; c->pk_cap_b = c->pk_cap_q = c->npos_cap = 0;
-}
-
 extern "C" void fp_ctx_destroy(fp_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
@@ -466,20 +472,10 @@ extern "C" void fp_ctx_destroy(fp_ctx* c) {
     { ParamOwner& po = g_param_owner[c->device & 63]; std::lock_guard<std::mutex> lk(po.mu); if (po.owner == c) po.owner = nullptr; }
     if (c->params_ev) cudaEventDestroy(c->params_ev);
     if (c->last_chain_ev) cudaEventDestroy(c->last_chain_ev);
-    free_staging(c);
-    {
-        fp_ctx::Buf* all[] = {&c->fq_term, &c->fq_bcnt, &c->fq_agg, &c->fq_bstate, &c->fq_brec, &c->fq_recline, &c->fq_recend, &c->fq_info, &c->fq_bsum,
-                              &c->fqh_text[0], &c->fqh_text[1], &c->fqh_seq[0], &c->fqh_seq[1], &c->fqh_qual[0], &c->fqh_qual[1], &c->fqh_len[0], &c->fqh_len[1],
-                              &c->fqh_recs[0], &c->fqh_recs[1], &c->fqh_res[0], &c->fqh_res[1], &c->fqh_ov, &c->fqh_out[0], &c->fqh_out[1],
-                              &c->fqh_recend[0], &c->fqh_recend[1], &c->fq_dupflags, &c->fqh_ovx};
-        for (auto& round : c->fqh_outbuf) for (auto& b : round) fq_free(b);
-        if (c->dup.bits) cudaFree(c->dup.bits);
-        cudaFree(c->d_dup_primes); cudaFree(c->d_dup_count);
-        fq_free(c->dup_pos); fq_free(c->dup_keys); fq_free(c->dup_vals);
-        if (c->fq_hinfo) cudaFreeHost(c->fq_hinfo);
-        if (c->fq_stream_out) { cudaStreamDestroy(c->fq_stream_out); cudaEventDestroy(c->fq_ev_up); cudaEventDestroy(c->fq_ev_out[0]); cudaEventDestroy(c->fq_ev_out[1]); }
-        for (auto* b : all) fq_free(*b);
-    }
+    if (c->dup.bits) cudaFree(c->dup.bits);
+    cudaFree(c->d_dup_primes); cudaFree(c->d_dup_count);
+    if (c->fq_hinfo) cudaFreeHost(c->fq_hinfo);
+    if (c->fq_stream_out) { cudaStreamDestroy(c->fq_stream_out); cudaEventDestroy(c->fq_ev_up); cudaEventDestroy(c->fq_ev_out[0]); cudaEventDestroy(c->fq_ev_out[1]); }
     cudaFree(c->d_dp);
     cudaFree(c->d_ovlimit); cudaFree(c->d_lowq); cudaFree(c->d_mindiff); cudaFree(c->d_adapters);
     cudaFree(c->d_fasta_off); cudaFree(c->d_fasta_len); cudaFree(c->d_raw); cudaFree(c->d_fin);
@@ -491,7 +487,7 @@ extern "C" void fp_ctx_destroy(fp_ctx* c) {
     for (auto& e : c->ev_pool) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
     for (int i = 0; i < 2; i++) if (c->stream[i]) cudaStreamDestroy(c->stream[i]);
     for (int i = 0; i < 4; i++) if (c->chunk_done[i]) cudaEventDestroy(c->chunk_done[i]);
-    delete c;
+    delete c;                                                  /* frees the staging and workspace buffers (Mem), on c->device set above */
 }
 
 extern "C" int fp_ctx_layout(const fp_ctx* c, fp_counter_layout* out) {
@@ -853,22 +849,45 @@ static int ensure_staging(fp_ctx* c) {
     const int sides = c->p.paired ? 2 : 1;
     int64_t chunk = std::min<int64_t>(std::max<int64_t>(c->max_batch, 1), (int64_t)1 << 18);
     chunk = (chunk + c->tile - 1) / c->tile * c->tile;
-    c->chunk = chunk;
     c->patch_cap = (uint32_t)std::min<int64_t>(chunk * 2 + 1024, (int64_t)1 << 22);
     for (int i = 0; i < 2; i++) {
-        for (int k = 0; k < 2 * sides; k++) CK(cudaMalloc(&c->d_stage[i][k], (size_t)chunk * c->stride + 64));
-        for (int k = 0; k < sides; k++) { CK(cudaMalloc(&c->d_stage_len[i][k], (size_t)chunk * 2)); CK(cudaMalloc(&c->d_out[i][k], (size_t)chunk * sizeof(fp_read_result))); }
+        for (int k = 0; k < 2 * sides; k++) CK(grow(c->d_stage[i][k], (size_t)chunk * c->stride + 64));
+        for (int k = 0; k < sides; k++) { CK(grow(c->d_stage_len[i][k], (size_t)chunk * 2)); CK(grow(c->d_out[i][k], (size_t)chunk * sizeof(fp_read_result))); }
         if (c->p.paired) {
-            CK(cudaMalloc(&c->d_ov[i], (size_t)chunk * sizeof(fp_ov_result)));
-            CK(cudaMalloc(&c->d_patch[i], (size_t)c->patch_cap * sizeof(fp_patch)));
-            CK(cudaMalloc(&c->d_npatch[i], 4));
+            CK(grow(c->d_ov[i], (size_t)chunk * sizeof(fp_ov_result)));
+            CK(grow(c->d_patch[i], (size_t)c->patch_cap * sizeof(fp_patch)));
+            CK(grow(c->d_npatch[i], 4));
         }
     }
     if (c->p.paired)
         for (int i = 0; i < 4; i++) {
-            CK(cudaMallocHost(&c->h_patch[i], (size_t)c->patch_cap * sizeof(fp_patch)));
-            CK(cudaMallocHost(&c->h_npatch[i], 4));
+            CK(grow(c->h_patch[i], (size_t)c->patch_cap * sizeof(fp_patch)));
+            CK(grow(c->h_npatch[i], 4));
         }
+    c->chunk = chunk;                                          /* only now: after a failed allocation the next call tries again */
+    return FP_OK;
+}
+
+/* one chunk of packed rows up, then small kernels restore the stride rows in HBM (6 TB/s: nothing next to the PCIe transfer) and put
+   back the 'N' bases of the chunk's exception list np[0 .. nn), whose units count from unit0 */
+static int upload_packed(fp_ctx* c, int slot, cudaStream_t st, int64_t cnt, const uint8_t* const bases[2], int pitch_b,
+                         const uint8_t* const qual[2], int pitch_q, const fp_npos* np, int64_t nn, int64_t unit0) {
+    const int S = c->stride, sides = c->p.paired ? 2 : 1;
+    if (nn > 0)
+        for (auto& d : c->d_npos) CK(grow_idle(d, (size_t)nn * sizeof(fp_npos), (size_t)(nn / 2 + 1024) * sizeof(fp_npos)));
+    for (int sd = 0; sd < sides; sd++) {
+        CK(cudaMemcpyAsync(c->d_pk[slot][2 * sd].p, bases[sd], (size_t)cnt * pitch_b, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(c->d_pk[slot][2 * sd + 1].p, qual[sd], (size_t)cnt * pitch_q, cudaMemcpyHostToDevice, st));
+    }
+    const long long thr = (long long)cnt * (S >> 4);
+    for (int sd = 0; sd < sides; sd++)
+        fp_unpack_kernel<<<(unsigned)((thr + 255) / 256), 256, 0, st>>>(c->d_pk[slot][2 * sd].p, c->d_pk[slot][2 * sd + 1].p, c->d_stage_len[slot][sd].p, cnt,
+                                                                       pitch_b, pitch_q, S, c->d_stage[slot][2 * sd].p, c->d_stage[slot][2 * sd + 1].p);
+    if (nn > 0) {
+        CK(cudaMemcpyAsync(c->d_npos[slot].p, np, (size_t)nn * sizeof(fp_npos), cudaMemcpyHostToDevice, st));
+        fp_unpack_n_kernel<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>(c->d_npos[slot].p, nn, unit0, S, c->d_stage[slot][0].p, sides == 2 ? c->d_stage[slot][2].p : nullptr);
+    }
+    CK(cudaGetLastError());
     return FP_OK;
 }
 
@@ -890,57 +909,33 @@ static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
     const bool repitch = !pk && !packfly && HP != c->stride;
     const int PB = ((((HP + 3) >> 2) + 3) & ~3);                 /* packed bases of one row, FP_B_PACK2BIT */
     const int NS = 4;                                          /* host staging slots of the packing team */
-    if (packfly) {
-        const size_t nb = (size_t)c->chunk * PB + 64, nq = (size_t)c->chunk * HP + 64;
-        if (nb > c->pk_cap_b || nq > c->pk_cap_q) {
-            CK(cudaDeviceSynchronize());
-            for (int i = 0; i < 2; i++)
-                for (int k = 0; k < (c->p.paired ? 4 : 2); k++) { cudaFree(c->d_pk[i][k]); c->d_pk[i][k] = nullptr; CK(cudaMalloc(&c->d_pk[i][k], (k & 1) ? nq : nb)); }
-            c->pk_cap_b = nb; c->pk_cap_q = nq;
-        }
-        if (nb > c->h_pkb_cap) {
-            for (int i = 0; i < NS; i++)
-                for (int k = 0; k < (c->p.paired ? 2 : 1); k++) { if (c->h_pkb[i][k]) cudaFreeHost(c->h_pkb[i][k]); c->h_pkb[i][k] = nullptr; CK(cudaMallocHost(&c->h_pkb[i][k], nb)); }
-            c->h_pkb_cap = nb;
-        }
-    }
-    if (repitch) {
-        const size_t nb = (size_t)c->chunk * HP + 64;
-        if (nb > c->pk_cap_b || nb > c->pk_cap_q) {
-            CK(cudaDeviceSynchronize());
-            for (int i = 0; i < 2; i++)
-                for (int k = 0; k < (c->p.paired ? 4 : 2); k++) { cudaFree(c->d_pk[i][k]); c->d_pk[i][k] = nullptr; CK(cudaMalloc(&c->d_pk[i][k], nb)); }
-            c->pk_cap_b = c->pk_cap_q = nb;
-        }
-    }
-    if (pk) {                                                  /* packed input: staging for one chunk of packed rows + its N exceptions */
-        if (pk->pitch_b <= 0 || pk->pitch_q <= 0) return set_err(FP_E_INVAL, "bad packed pitch");
-        const size_t nb = (size_t)c->chunk * pk->pitch_b + 64, nq = (size_t)c->chunk * pk->pitch_q + 64;
-        if (nb > c->pk_cap_b || nq > c->pk_cap_q) {
-            CK(cudaDeviceSynchronize());
-            for (int i = 0; i < 2; i++)
-                for (int k = 0; k < (c->p.paired ? 4 : 2); k++) { cudaFree(c->d_pk[i][k]); CK(cudaMalloc(&c->d_pk[i][k], (k & 1) ? nq : nb)); }
-            c->pk_cap_b = nb; c->pk_cap_q = nq;
-        }
-    }
     const bool pe = c->p.paired;
-    const int S = c->stride;
+    const int S = c->stride, sides = pe ? 2 : 1;
     const int64_t n = b->n, CH = c->chunk;
     const int64_t nchunks = (n + CH - 1) / CH;
+    /* rows not at the device stride go up into d_pk at the format's pitches (bases, qualities), then a kernel puts them at the stride */
+    if (pk && (pk->pitch_b <= 0 || pk->pitch_q <= 0)) return set_err(FP_E_INVAL, "bad packed pitch");
+    const int pitch_b = pk ? pk->pitch_b : packfly ? PB : HP, pitch_q = pk ? pk->pitch_q : HP;
+    if (pk || packfly || repitch)
+        for (auto& s : c->d_pk)
+            for (int k = 0; k < 2 * sides; k++) CK(grow_idle(s[k], (size_t)CH * ((k & 1) ? pitch_q : pitch_b) + 64));
+    if (packfly)
+        for (auto& s : c->h_pkb)
+            for (int k = 0; k < sides; k++) CK(grow_idle(s[k], (size_t)CH * PB + 64));
+    const uint8_t* const rows[4] = {b->seq1, b->qual1, b->seq2, b->qual2};                 /* the caller's rows at pitch HP */
+    const uint16_t* const lens[2] = {pk ? pk->len1 : b->len1, pk ? pk->len2 : b->len2};
     struct Pending { int64_t lo, cnt; bool active; } pend[4] = {{0, 0, false}, {0, 0, false}, {0, 0, false}, {0, 0, false}};   /* by chunk % 4 */
     const bool want_ev = c->ev_host_n != nullptr;
     if (want_ev) {
         *c->ev_host_n = 0;
-        if (!c->d_ev[0]) {
-            /* a pair gives at most 2 events (trimByOverlapAnalysis, or trimBySequence on each read) + 1 per fasta adapter and read; a read
-               1 + 1 per fasta adapter.  Past 2^24 entries (a full chunk with more than 30 fasta adapters PE, 62 SE) a chunk could still
-               overflow: finish() fails then */
-            const int64_t per_unit = pe ? 2 + 2 * (int64_t)c->p.n_fasta_adapters : 1 + (int64_t)c->p.n_fasta_adapters;
-            c->ev_chunk_cap = (uint32_t)std::min<int64_t>(CH * per_unit + 1024, (int64_t)1 << 24);
-            for (int i = 0; i < 2; i++) {
-                CK(cudaMalloc(&c->d_ev[i], (size_t)c->ev_chunk_cap * sizeof(fp_adapter_event))); CK(cudaMalloc(&c->d_nev[i], 4));
-                CK(cudaMallocHost(&c->h_ev[i], (size_t)c->ev_chunk_cap * sizeof(fp_adapter_event))); CK(cudaMallocHost(&c->h_nev[i], 4));
-            }
+        /* a pair gives at most 2 events (trimByOverlapAnalysis, or trimBySequence on each read) + 1 per fasta adapter and read; a read
+           1 + 1 per fasta adapter.  Past 2^24 entries (a full chunk with more than 30 fasta adapters PE, 62 SE) a chunk could still
+           overflow: finish() fails then */
+        const int64_t per_unit = pe ? 2 + 2 * (int64_t)c->p.n_fasta_adapters : 1 + (int64_t)c->p.n_fasta_adapters;
+        c->ev_chunk_cap = (uint32_t)std::min<int64_t>(CH * per_unit + 1024, (int64_t)1 << 24);
+        for (int i = 0; i < 2; i++) {                          /* the same sizes on every call: grow() only replaces what is missing */
+            CK(grow(c->d_ev[i], (size_t)c->ev_chunk_cap * sizeof(fp_adapter_event))); CK(grow(c->d_nev[i], 4));
+            CK(grow(c->h_ev[i], (size_t)c->ev_chunk_cap * sizeof(fp_adapter_event))); CK(grow(c->h_nev[i], 4));
         }
     }
     /* the device sink of fp_set_event_sink (if any) is put back when this call returns */
@@ -957,23 +952,23 @@ static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
         CK(cudaEventSynchronize(c->chunk_done[hs]));             /* blocking-sync event: the waiting thread sleeps instead of spinning.  One event per
                                                                     chunk in flight on the HOST side (k % 4): the slot's next chunk records its own */
         if (want_ev) {
-            const uint32_t ne = *c->h_nev[slot];
+            const uint32_t ne = *c->h_nev[slot].p;
             /* the kernel dropped what did not fit: the caller's list would have a hole in the middle */
             if (ne > c->ev_chunk_cap) return set_err(FP_E_TOOLARGE, "adapter events of one host chunk exceed its event buffer (too many fasta adapters)");
-            if (ne > 0) CK(cudaMemcpy(c->h_ev[slot], c->d_ev[slot], (size_t)ne * sizeof(fp_adapter_event), cudaMemcpyDeviceToHost));
+            if (ne > 0) CK(cudaMemcpy(c->h_ev[slot].p, c->d_ev[slot].p, (size_t)ne * sizeof(fp_adapter_event), cudaMemcpyDeviceToHost));
             for (uint32_t i = 0; i < ne; i++) {
-                if (*c->ev_host_n < c->ev_host_cap) { c->ev_host[*c->ev_host_n] = c->h_ev[slot][i]; c->ev_host[*c->ev_host_n].unit = (uint32_t)(pend[hs].lo + c->h_ev[slot][i].unit); }
+                if (*c->ev_host_n < c->ev_host_cap) { c->ev_host[*c->ev_host_n] = c->h_ev[slot].p[i]; c->ev_host[*c->ev_host_n].unit = (uint32_t)(pend[hs].lo + c->h_ev[slot].p[i].unit); }
                 (*c->ev_host_n)++;
             }
         }
         if (pe && c->p.correction_enabled) {
-            uint32_t np = *c->h_npatch[hs];
+            uint32_t np = *c->h_npatch[hs].p;
             const int64_t lo = pend[hs].lo;
             if (np <= c->patch_cap) {
                 /* the write-back touches two random cache lines per correction: memory-latency bound (16 ns per patch on one core, 3 ms per
                    chunk -- more than the chunk's transfer).  The lines of the patch 24 entries ahead are requested while this one is
                    applied, and a large list is split over four threads (no two patches touch the same byte). */
-                const fp_patch* const P = c->h_patch[hs];
+                const fp_patch* const P = c->h_patch[hs].p;
                 if (!pk) {
                     auto apply_range = [&](uint32_t a0, uint32_t a1) {
                         for (uint32_t i = a0; i < a1; i++) {
@@ -1008,7 +1003,7 @@ static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
                 if (hp_n) *hp_n = ~(uint64_t)0 >> 1;             /* the caller's list cannot be complete */
                 uint8_t* dst[4] = {b->seq1, b->qual1, b->seq2, b->qual2};
                 for (int a4 = 0; a4 < 4; a4++)
-                    CK(cudaMemcpy2D(dst[a4] + lo * HP, (size_t)HP, c->d_stage[slot][a4], (size_t)S, (size_t)HP, (size_t)pend[hs].cnt, cudaMemcpyDeviceToHost));
+                    CK(cudaMemcpy2D(dst[a4] + lo * HP, (size_t)HP, c->d_stage[slot][a4].p, (size_t)S, (size_t)HP, (size_t)pend[hs].cnt, cudaMemcpyDeviceToHost));
             }
         }
         pend[hs].active = false;
@@ -1034,7 +1029,6 @@ static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
         team.allowed = 1;
         for (int t = 0; t < NT; t++)
             team.th.emplace_back([&, t]() {
-                const int sides = pe ? 2 : 1;
                 for (int64_t k = 0; k < nchunks; k++) {
                     {
                         std::unique_lock<std::mutex> lk(team.mu);
@@ -1049,7 +1043,7 @@ static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
                         for (int sd = 0; sd < sides; sd++) {
                             const int L = (sd ? b->len2 : b->len1)[lo + r];
                             if (L > HP) { team.bad.store(2); break; }
-                            if (fp_pack_bases_row((sd ? b->seq2 : b->seq1) + (lo + r) * HP, L, c->h_pkb[k % NS][sd] + r * PB, (uint32_t)r, sd, nl)) { team.bad.store(1); break; }
+                            if (fp_pack_bases_row((sd ? b->seq2 : b->seq1) + (lo + r) * HP, L, c->h_pkb[k % NS][sd].p + r * PB, (uint32_t)r, sd, nl)) { team.bad.store(1); break; }
                         }
                     bool last;
                     { std::lock_guard<std::mutex> lk(team.mu); last = ++team.done[(size_t)k] == NT; }
@@ -1111,7 +1105,7 @@ static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
             const int64_t k2 = ci - 2;
             CK(cudaEventSynchronize(c->chunk_done[k2 & 3]));
             t_slot += ms_since(tp); tp = now();
-            const bool needs_dev = want_ev || (pe && c->p.correction_enabled && *c->h_npatch[k2 & 3] > c->patch_cap);
+            const bool needs_dev = want_ev || (pe && c->p.correction_enabled && *c->h_npatch[k2 & 3].p > c->patch_cap);
             rc = fin_wait(needs_dev ? ci - 1 : std::max<int64_t>(ci - 3, 0));
             t_fin += ms_since(tp); tp = now();
         }
@@ -1126,123 +1120,67 @@ static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
         }
         const int64_t lo = ci * CH, cnt = std::min(CH, n - lo);
         cudaStream_t st = c->stream[slot];
-        const size_t bytes = (size_t)cnt * S;
-        if (pk) {
-            /* packed rows up, then a small kernel restores the stride rows in HBM (6 TB/s: nothing next to the PCIe transfer) */
-            const size_t bb = (size_t)cnt * pk->pitch_b, qb = (size_t)cnt * pk->pitch_q;
-            CK(cudaMemcpyAsync(c->d_pk[slot][0], pk->bases1 + lo * pk->pitch_b, bb, cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(c->d_pk[slot][1], pk->qual1 + lo * pk->pitch_q, qb, cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(c->d_stage_len[slot][0], pk->len1 + lo, (size_t)cnt * 2, cudaMemcpyHostToDevice, st));
-            if (pe) {
-                CK(cudaMemcpyAsync(c->d_pk[slot][2], pk->bases2 + lo * pk->pitch_b, bb, cudaMemcpyHostToDevice, st));
-                CK(cudaMemcpyAsync(c->d_pk[slot][3], pk->qual2 + lo * pk->pitch_q, qb, cudaMemcpyHostToDevice, st));
-                CK(cudaMemcpyAsync(c->d_stage_len[slot][1], pk->len2 + lo, (size_t)cnt * 2, cudaMemcpyHostToDevice, st));
-                CK(cudaMemsetAsync(c->d_npatch[slot], 0, 4, st));
+        for (int sd = 0; sd < sides; sd++) CK(cudaMemcpyAsync(c->d_stage_len[slot][sd].p, lens[sd] + lo, (size_t)cnt * 2, cudaMemcpyHostToDevice, st));
+        if (pe) CK(cudaMemsetAsync(c->d_npatch[slot].p, 0, 4, st));
+        if (pk || packfly) {
+            const uint8_t* bases[2] = {}; const uint8_t* qual[2] = {};
+            const fp_npos* np; int64_t nn, unit0;
+            if (pk) {                                          /* the chunk's slice of the caller's sorted 'N' list */
+                auto unit_less = [](const fp_npos& e, uint32_t v) { return e.unit < v; };
+                np = std::lower_bound(pk->npos, pk->npos + pk->n_npos, (uint32_t)lo, unit_less);
+                nn = std::lower_bound(np, (const fp_npos*)(pk->npos + pk->n_npos), (uint32_t)(lo + cnt), unit_less) - np;
+                unit0 = lo;
+                bases[0] = pk->bases1 + lo * pitch_b; qual[0] = pk->qual1 + lo * pitch_q;
+                if (pe) { bases[1] = pk->bases2 + lo * pitch_b; qual[1] = pk->qual2 + lo * pitch_q; }
+            } else {                                           /* the packing team's lists of this chunk, gathered into its pinned slot */
+                const int hs = (int)(ci % NS);
+                size_t m = 0;
+                for (int t = 0; t < NT; t++) m += team.nl[(size_t)t * NS + hs].size();
+                for (auto& h : c->h_np) CK(grow_idle(h, m * sizeof(fp_npos), (m / 2 + 4096) * sizeof(fp_npos)));
+                size_t o = 0;
+                for (int t = 0; t < NT; t++) { const auto& v = team.nl[(size_t)t * NS + hs]; if (!v.empty()) memcpy(c->h_np[hs].p + o, v.data(), v.size() * sizeof(fp_npos)); o += v.size(); }
+                np = c->h_np[hs].p; nn = (int64_t)m; unit0 = 0;
+                for (int sd = 0; sd < sides; sd++) { bases[sd] = c->h_pkb[hs][sd].p; qual[sd] = rows[2 * sd + 1] + lo * HP; }
             }
-            const long long thr = (long long)cnt * (S >> 4);
-            fp_unpack_kernel<<<(unsigned)((thr + 255) / 256), 256, 0, st>>>(c->d_pk[slot][0], c->d_pk[slot][1], c->d_stage_len[slot][0], cnt, pk->pitch_b, pk->pitch_q, S,
-                                                                          c->d_stage[slot][0], c->d_stage[slot][1]);
-            if (pe) fp_unpack_kernel<<<(unsigned)((thr + 255) / 256), 256, 0, st>>>(c->d_pk[slot][2], c->d_pk[slot][3], c->d_stage_len[slot][1], cnt, pk->pitch_b, pk->pitch_q, S,
-                                                                                  c->d_stage[slot][2], c->d_stage[slot][3]);
-            /* the chunk's slice of the sorted 'N' list */
-            const fp_npos* nb0 = std::lower_bound(pk->npos, pk->npos + pk->n_npos, (uint32_t)lo, [](const fp_npos& e, uint32_t v) { return e.unit < v; });
-            const fp_npos* nb1 = std::lower_bound(nb0, (const fp_npos*)(pk->npos + pk->n_npos), (uint32_t)(lo + cnt), [](const fp_npos& e, uint32_t v) { return e.unit < v; });
-            const long long nn = nb1 - nb0;
-            if (nn > 0) {
-                if ((size_t)nn > c->npos_cap) {
-                    CK(cudaDeviceSynchronize());
-                    for (int i = 0; i < 2; i++) { cudaFree(c->d_npos[i]); CK(cudaMalloc(&c->d_npos[i], (size_t)(nn + nn / 2 + 1024) * sizeof(fp_npos))); }
-                    c->npos_cap = (size_t)(nn + nn / 2 + 1024);
-                }
-                CK(cudaMemcpyAsync(c->d_npos[slot], nb0, (size_t)nn * sizeof(fp_npos), cudaMemcpyHostToDevice, st));
-                fp_unpack_n_kernel<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>(c->d_npos[slot], nn, lo, S, c->d_stage[slot][0], pe ? c->d_stage[slot][2] : nullptr);
-            }
-            CK(cudaGetLastError());
-        } else if (packfly) {
-            const int hs = (int)(ci % NS);
-            size_t nn = 0;
-            for (int t = 0; t < NT; t++) nn += team.nl[(size_t)t * NS + hs].size();
-            if (nn > c->h_np_cap) {                                /* the slots' older chunks are done (finish above): safe to re-allocate */
-                CK(cudaDeviceSynchronize());
-                const size_t cap = nn + nn / 2 + 4096;
-                for (int i = 0; i < NS; i++) { if (c->h_np[i]) cudaFreeHost(c->h_np[i]); c->h_np[i] = nullptr; CK(cudaMallocHost(&c->h_np[i], cap * sizeof(fp_npos))); }
-                c->h_np_cap = cap;
-            }
-            if (nn > c->npos_cap) {
-                CK(cudaDeviceSynchronize());
-                for (int i = 0; i < 2; i++) { cudaFree(c->d_npos[i]); c->d_npos[i] = nullptr; CK(cudaMalloc(&c->d_npos[i], (nn + nn / 2 + 1024) * sizeof(fp_npos))); }
-                c->npos_cap = nn + nn / 2 + 1024;
-            }
-            size_t o = 0;
-            for (int t = 0; t < NT; t++) { const auto& v = team.nl[(size_t)t * NS + hs]; if (!v.empty()) memcpy(c->h_np[hs] + o, v.data(), v.size() * sizeof(fp_npos)); o += v.size(); }
-            const size_t bb = (size_t)cnt * PB, qb = (size_t)cnt * HP;
-            CK(cudaMemcpyAsync(c->d_pk[slot][0], c->h_pkb[hs][0], bb, cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(c->d_pk[slot][1], b->qual1 + lo * HP, qb, cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(c->d_stage_len[slot][0], b->len1 + lo, (size_t)cnt * 2, cudaMemcpyHostToDevice, st));
-            if (pe) {
-                CK(cudaMemcpyAsync(c->d_pk[slot][2], c->h_pkb[hs][1], bb, cudaMemcpyHostToDevice, st));
-                CK(cudaMemcpyAsync(c->d_pk[slot][3], b->qual2 + lo * HP, qb, cudaMemcpyHostToDevice, st));
-                CK(cudaMemcpyAsync(c->d_stage_len[slot][1], b->len2 + lo, (size_t)cnt * 2, cudaMemcpyHostToDevice, st));
-                CK(cudaMemsetAsync(c->d_npatch[slot], 0, 4, st));
-            }
-            const long long thr = (long long)cnt * (S >> 4);
-            fp_unpack_kernel<<<(unsigned)((thr + 255) / 256), 256, 0, st>>>(c->d_pk[slot][0], c->d_pk[slot][1], c->d_stage_len[slot][0], cnt, PB, HP, S, c->d_stage[slot][0], c->d_stage[slot][1]);
-            if (pe) fp_unpack_kernel<<<(unsigned)((thr + 255) / 256), 256, 0, st>>>(c->d_pk[slot][2], c->d_pk[slot][3], c->d_stage_len[slot][1], cnt, PB, HP, S, c->d_stage[slot][2], c->d_stage[slot][3]);
-            if (nn > 0) {
-                CK(cudaMemcpyAsync(c->d_npos[slot], c->h_np[hs], nn * sizeof(fp_npos), cudaMemcpyHostToDevice, st));
-                fp_unpack_n_kernel<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>(c->d_npos[slot], (long long)nn, 0, S, c->d_stage[slot][0], pe ? c->d_stage[slot][2] : nullptr);
-            }
-            CK(cudaGetLastError());
+            if ((rc = upload_packed(c, slot, st, cnt, bases, pitch_b, qual, pitch_q, np, nn, unit0))) return rc;
         } else if (repitch) {
-            const size_t hb = (size_t)cnt * HP;
-            const uint8_t* src[4] = {b->seq1, b->qual1, b->seq2, b->qual2};
-            CK(cudaMemcpyAsync(c->d_stage_len[slot][0], b->len1 + lo, (size_t)cnt * 2, cudaMemcpyHostToDevice, st));
-            if (pe) { CK(cudaMemcpyAsync(c->d_stage_len[slot][1], b->len2 + lo, (size_t)cnt * 2, cudaMemcpyHostToDevice, st)); CK(cudaMemsetAsync(c->d_npatch[slot], 0, 4, st)); }
             const long long thr = (long long)cnt * (S >> 4);
-            for (int k = 0; k < (pe ? 4 : 2); k++) {
-                CK(cudaMemcpyAsync(c->d_pk[slot][k], src[k] + lo * HP, hb, cudaMemcpyHostToDevice, st));
-                fp_repitch_kernel<<<(unsigned)((thr + 255) / 256), 256, 0, st>>>(c->d_pk[slot][k], c->d_stage_len[slot][k >> 1], cnt, HP, S, c->d_stage[slot][k]);
+            for (int k = 0; k < 2 * sides; k++) {
+                CK(cudaMemcpyAsync(c->d_pk[slot][k].p, rows[k] + lo * HP, (size_t)cnt * HP, cudaMemcpyHostToDevice, st));
+                fp_repitch_kernel<<<(unsigned)((thr + 255) / 256), 256, 0, st>>>(c->d_pk[slot][k].p, c->d_stage_len[slot][k >> 1].p, cnt, HP, S, c->d_stage[slot][k].p);
             }
             CK(cudaGetLastError());
         } else {
-        CK(cudaMemcpyAsync(c->d_stage[slot][0], b->seq1 + lo * S, bytes, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(c->d_stage[slot][1], b->qual1 + lo * S, bytes, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(c->d_stage_len[slot][0], b->len1 + lo, (size_t)cnt * 2, cudaMemcpyHostToDevice, st));
-        if (pe) {
-            CK(cudaMemcpyAsync(c->d_stage[slot][2], b->seq2 + lo * S, bytes, cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(c->d_stage[slot][3], b->qual2 + lo * S, bytes, cudaMemcpyHostToDevice, st));
-            CK(cudaMemcpyAsync(c->d_stage_len[slot][1], b->len2 + lo, (size_t)cnt * 2, cudaMemcpyHostToDevice, st));
-            CK(cudaMemsetAsync(c->d_npatch[slot], 0, 4, st));
-        }
+            for (int k = 0; k < 2 * sides; k++) CK(cudaMemcpyAsync(c->d_stage[slot][k].p, rows[k] + lo * S, (size_t)cnt * S, cudaMemcpyHostToDevice, st));
         }
         if (want_ev) {
-            CK(cudaMemsetAsync(c->d_nev[slot], 0, 4, st));
-            c->ev_dev = c->d_ev[slot]; c->ev_cap = c->ev_chunk_cap; c->ev_count = c->d_nev[slot];
+            CK(cudaMemsetAsync(c->d_nev[slot].p, 0, 4, st));
+            c->ev_dev = c->d_ev[slot].p; c->ev_cap = c->ev_chunk_cap; c->ev_count = c->d_nev[slot].p;
         }
         fp_batch db;
         memset(&db, 0, sizeof(db));
         db.n = cnt; db.stride = S;
         if (b->flags & FP_B_INDEXED) { db.flags = FP_B_INDEXED; db.first_read_index = b->first_read_index + lo; }
-        db.seq1 = c->d_stage[slot][0]; db.qual1 = c->d_stage[slot][1]; db.len1 = c->d_stage_len[slot][0];
-        if (pe) { db.seq2 = c->d_stage[slot][2]; db.qual2 = c->d_stage[slot][3]; db.len2 = c->d_stage_len[slot][1]; }
+        db.seq1 = c->d_stage[slot][0].p; db.qual1 = c->d_stage[slot][1].p; db.len1 = c->d_stage_len[slot][0].p;
+        if (pe) { db.seq2 = c->d_stage[slot][2].p; db.qual2 = c->d_stage[slot][3].p; db.len2 = c->d_stage_len[slot][1].p; }
         /* the over-representation sampling state (running counts, rank scratch) is one per ctx: chunk k+1's kernels wait for chunk
            k's (its H2D copies, issued above, still overlap them) */
         if (c->p.overrep_enabled) {
             if (!c->ovr_ev) CK(cudaEventCreateWithFlags(&c->ovr_ev, cudaEventDisableTiming));
             else CK(cudaStreamWaitEvent(st, c->ovr_ev, 0));
         }
-        rc = launch_chain(c, &db, c->d_out[slot][0], pe ? c->d_out[slot][1] : nullptr, pe ? c->d_ov[slot] : nullptr,
-                          pe ? c->d_patch[slot] : nullptr, c->patch_cap, pe ? c->d_npatch[slot] : nullptr, st);
+        rc = launch_chain(c, &db, c->d_out[slot][0].p, pe ? c->d_out[slot][1].p : nullptr, pe ? c->d_ov[slot].p : nullptr,
+                          pe ? c->d_patch[slot].p : nullptr, c->patch_cap, pe ? c->d_npatch[slot].p : nullptr, st);
         if (rc) return rc;
         if (c->p.overrep_enabled) CK(cudaEventRecord(c->ovr_ev, st));
-        if (want_ev) CK(cudaMemcpyAsync(c->h_nev[slot], c->d_nev[slot], 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(out1 + lo, c->d_out[slot][0], (size_t)cnt * sizeof(fp_read_result), cudaMemcpyDeviceToHost, st));
+        if (want_ev) CK(cudaMemcpyAsync(c->h_nev[slot].p, c->d_nev[slot].p, 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(out1 + lo, c->d_out[slot][0].p, (size_t)cnt * sizeof(fp_read_result), cudaMemcpyDeviceToHost, st));
         if (pe) {
-            CK(cudaMemcpyAsync(out2 + lo, c->d_out[slot][1], (size_t)cnt * sizeof(fp_read_result), cudaMemcpyDeviceToHost, st));
-            if (ov) CK(cudaMemcpyAsync(ov + lo, c->d_ov[slot], (size_t)cnt * sizeof(fp_ov_result), cudaMemcpyDeviceToHost, st));
+            CK(cudaMemcpyAsync(out2 + lo, c->d_out[slot][1].p, (size_t)cnt * sizeof(fp_read_result), cudaMemcpyDeviceToHost, st));
+            if (ov) CK(cudaMemcpyAsync(ov + lo, c->d_ov[slot].p, (size_t)cnt * sizeof(fp_ov_result), cudaMemcpyDeviceToHost, st));
             if (c->p.correction_enabled) {
-                CK(cudaMemcpyAsync(c->h_npatch[ci & 3], c->d_npatch[slot], 4, cudaMemcpyDeviceToHost, st));
-                CK(cudaMemcpyAsync(c->h_patch[ci & 3], c->d_patch[slot], (size_t)c->patch_cap * sizeof(fp_patch), cudaMemcpyDeviceToHost, st));
+                CK(cudaMemcpyAsync(c->h_npatch[ci & 3].p, c->d_npatch[slot].p, 4, cudaMemcpyDeviceToHost, st));
+                CK(cudaMemcpyAsync(c->h_patch[ci & 3].p, c->d_patch[slot].p, (size_t)c->patch_cap * sizeof(fp_patch), cudaMemcpyDeviceToHost, st));
             }
         }
         CK(cudaEventRecord(c->chunk_done[ci & 3], st));
@@ -1297,12 +1235,7 @@ extern "C" int fp_process_pe_host_patches(fp_ctx* c, const fp_batch* b, fp_read_
 
 /* ---------------- FASTQ text <-> rows (fp_fastq.cuh) ---------------- */
 static int fq_ensure(fp_ctx::Buf& b, size_t need) {
-    if (need <= b.cap) return FP_OK;
-    if (b.p) cudaFree(b.p);
-    b.p = nullptr; b.cap = 0;
-    size_t cap = need + need / 4 + 256;
-    CK(cudaMalloc(&b.p, cap));
-    b.cap = cap;
+    CK(grow(b, need, need / 4 + 256));
     return FP_OK;
 }
 

@@ -86,16 +86,24 @@ def test_counters_accumulate_over_three_launches(gpu, name, paired):
 
 
 # ---------------- host entry points ----------------
-@pytest.mark.parametrize("mode", ["host", "host_tight", "host_pack2bit", "packed"])
+@pytest.mark.parametrize("mode,max_batch", [pytest.param(m, mb, id=m if mb is None else f"{m}-max_batch{mb}")
+                                            for mb in (None, 1024) for m in ("host", "host_tight", "host_pack2bit", "packed")])
 @pytest.mark.parametrize("name,paired", [("cfg4_full", 1), ("cfg3_overlap_correction", 1), ("all_cuts", 1), ("cfg4_full", 0), ("filters", 0)])
-def test_host_entry_points(gpu, name, paired, mode):
+def test_host_entry_points(gpu, name, paired, mode, max_batch):
     """The same inputs through fp_process_*_host at the device pitch, at the tight pitch of the longest read (150 of 160),
-    packed on the fly (FP_B_PACK2BIT) and packed by the caller (the rows hold A/C/G/T/N only)."""
+    packed on the fly (FP_B_PACK2BIT) and packed by the caller (the rows hold A/C/G/T/N only).  max_batch 1024: a ctx whose host
+    chunks hold 1024 units, so the 20000 units go through about 20 chunks (completion on the helper thread, the 'N' list sliced at
+    every chunk's offset) instead of one."""
     p, arrs = grid_input(name, paired, 160, n=20000, seed=17, max_len=150 if mode == "host_tight" else None)
     if mode == "host_tight":
         assert arrs["len1"].max() == 150
     want = T.run_cpu("oracle", p, arrs, 160)
-    T.assert_results_equal(gpu.run_gpu(p, arrs, 160, mode=mode), want, paired, what=f"{mode} {name}")
+    ctx = gpu.GpuCtx(p, max_batch, 160, 160) if max_batch else None
+    try:
+        T.assert_results_equal(gpu.run_gpu(p, arrs, 160, mode=mode, ctx=ctx), want, paired, what=f"{mode} {name} max_batch {max_batch}")
+    finally:
+        if ctx:
+            ctx.close()
 
 
 # ---------------- correction overflow on the device ----------------
