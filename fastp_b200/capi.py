@@ -88,7 +88,8 @@ class CounterLayout(C.Structure):
 # numpy views of the record structs
 READ_RESULT_DTYPE = np.dtype([
     ("front", "<u2"), ("len", "<u2"), ("verdict", "u1"), ("flags", "u1"), ("adapter_pos", "<i2"),
-    ("adapter_len", "<u2"), ("polyx_base", "u1"), ("pair_verdict", "u1"), ("polyx_len", "<u2"), ("reserved", "<u2"),
+    ("adapter_len", "<u2"), ("polyx_base", "u1"), ("pair_verdict", "u1"), ("polyx_len", "<u2"),
+    ("reserved", "<u2"),      # flags2 of the C struct (FP_F2_*): 0 unless the index filter is on, so it keeps its old column name here
 ])
 OV_RESULT_DTYPE = np.dtype([
     ("overlapped", "u1"), ("has_gap", "u1"), ("offset", "<i2"), ("overlap_len", "<i2"), ("diff", "<i2"),
@@ -195,6 +196,9 @@ SYMBOLS = {
     "fp_set_overlapped_sink": (C.c_int, [C.c_void_p, C.c_void_p]),
     "fp_fastq_encode_overlapped": (C.c_int, [C.c_void_p] + [C.c_void_p] * 7 + [C.c_int64, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]),
     "fp_fastq_set_overlapped_out": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]),
+    "fp_set_index_flags": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "fp_fastq_set_index_filter": (C.c_int, [C.c_void_p, C.POINTER(C.c_char_p), C.c_int64, C.POINTER(C.c_char_p), C.c_int64, C.c_int32]),
+    "fp_fastq_index_flags": (C.c_int, [C.c_void_p] + [C.c_void_p] * 4 + [C.c_int64, C.c_void_p]),
 }
 
 

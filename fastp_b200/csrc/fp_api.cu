@@ -159,6 +159,11 @@ struct fp_ctx {
     int fq_dup_level = 0, fq_dedup = 0;     /* fp_fastq_set_dedup */
     int fq_il_in = 0, fq_il_out = 0;        /* fp_fastq_set_interleaved */
     Buf fq_dupflags;
+    const uint8_t* ix_flags = nullptr;      /* fp_set_index_flags: index-filter flags of the batch the next launch works on */
+    /* fp_fastq_set_index_filter: the text path's barcode lists (fq_index_list layout) and the round's flags */
+    Buf fq_ix_words[2], fq_ix_lens[2], fq_ixflags;
+    int fq_ix_n[2] = {0, 0}, fq_ix_w[2] = {1, 1}, fq_ix_thr = 0;
+    bool fq_ix_on = false;
     Buf dup_pos, dup_keys, dup_vals;
     /* kernel timing */
     std::vector<EvPair> evs;
@@ -555,6 +560,7 @@ static int launch_chain(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
     a.sink.patches = patches; a.sink.cap = patches ? patch_cap : 0; a.sink.count = n_patches;
     a.is_dup = c->dup_flags;
     a.ovx = c->p.paired ? c->ovx : nullptr;
+    a.ix_flags = c->ix_flags;
     a.events.events = c->ev_dev; a.events.cap = c->ev_dev ? c->ev_cap : 0; a.events.count = c->ev_count;
     a.counters = reinterpret_cast<unsigned long long*>(c->d_raw);
     a.n_tiles = (b->n + c->tile - 1) / c->tile;
@@ -898,6 +904,7 @@ static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
     if (hp_n) *hp_n = 0;
     /* the chain indexes the flags by the unit's index in its LAUNCH, and a host batch is launched chunk by chunk */
     if (c->dup_flags) return set_err(FP_E_INVAL, "duplicate flags are set (fp_set_dup_flags): they belong to one fp_process_se / _pe launch, not to a host batch");
+    if (c->ix_flags) return set_err(FP_E_INVAL, "index-filter flags are set (fp_set_index_flags): they belong to one fp_process_se / _pe launch, not to a host batch");
     if (c->ovx) return set_err(FP_E_INVAL, "an overlapped sink is set (fp_set_overlapped_sink): it belongs to one fp_process_pe launch, not to a host batch");
     CK(cudaSetDevice(c->device));
     int rc = ensure_staging(c);
@@ -1452,6 +1459,19 @@ extern "C" int fp_fastq_encode_rejects(fp_ctx* c, int32_t which, int32_t writers
     return fastq_encode_impl<FQ_SEL_FAILED>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
 }
 
+/* Filter::filterByIndex over a batch of decoded records (fq_index_flags_kernel), enqueued on st */
+static int index_flags_launch(fp_ctx* c, const uint8_t* text1, const fq_rec* recs1, const uint8_t* text2, const fq_rec* recs2, int64_t n,
+                              uint8_t* flags, cudaStream_t st) {
+    if (n <= 0) return FP_OK;
+    if (!c->fq_ix_on) { CK(cudaMemsetAsync(flags, 0, (size_t)n, st)); return FP_OK; }
+    fq_index_list L[2];
+    for (int k = 0; k < 2; k++) { L[k].words = (const uint32_t*)c->fq_ix_words[k].p; L[k].lens = (const uint16_t*)c->fq_ix_lens[k].p; L[k].n = c->fq_ix_n[k]; L[k].W = c->fq_ix_w[k]; }
+    const long long blocks = std::min<long long>((n + FQ_IX_WARPS - 1) / FQ_IX_WARPS, (long long)c->num_sms * 64);
+    fq_index_flags_kernel<<<(unsigned)blocks, 32 * FQ_IX_WARPS, 0, st>>>(text1, recs1, c->p.paired ? text2 : nullptr, recs2, n, L[0], L[1], c->fq_ix_thr, flags);
+    CK(cudaGetLastError());
+    return FP_OK;
+}
+
 /* The round loop of the text path.  outs / ocap / out_bytes are indexed by FP_FQ_OUT_*; a NULL buffer is not encoded.  merging: the ctx
    merges pairs, so every round also keeps the chain's overlap results for the merged stream.  The reject streams read the round's decoded
    lengths (fqh_len, which the chain leaves as they are) and take the unpaired writers from which unpaired buffers are given.  The
@@ -1473,6 +1493,7 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
     const bool il_in = c->fq_il_in && sides == 2, il_out = c->fq_il_out && sides == 2 && !merging;
     if (c->dup_flags) return set_err(FP_E_INVAL, "duplicate flags are set (fp_set_dup_flags): the text path runs its own duplicate filter (fp_fastq_set_dedup)");
     if (c->ovx) return set_err(FP_E_INVAL, "an overlapped sink is set (fp_set_overlapped_sink): the text path keeps its own (fp_fastq_set_overlapped_out)");
+    if (c->ix_flags) return set_err(FP_E_INVAL, "index-filter flags are set (fp_set_index_flags): the text path runs its own index filter (fp_fastq_set_index_filter)");
     if (il_in && (text2 || nbytes2 != 0)) return set_err(FP_E_INVAL, "interleaved input: both mates are in text1 (pass text2 NULL and nbytes2 0)");
     if (il_out && outs[FP_FQ_OUT_R2]) return set_err(FP_E_INVAL, "interleaved output: both reads go to out1 (pass no out2 buffer)");
     CK(cudaSetDevice(c->device));
@@ -1502,6 +1523,7 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
     }
     if (merging && (rc = fq_ensure(c->fqh_ov, (size_t)cap * sizeof(fp_ov_result)))) return rc;
     if (ovx && (rc = fq_ensure(c->fqh_ovx, (size_t)cap * sizeof(fp_overlapped_result)))) return rc;
+    if (c->fq_ix_on && (rc = fq_ensure(c->fq_ixflags, (size_t)cap))) return rc;
     int64_t upl[2] = {0, 0}, start[2] = {0, 0}, obytes[NOUT] = {0}, units = 0;
     fp_fastq_info agg[2]; memset(agg, 0, sizeof(agg)); agg[0].error_record = agg[1].error_record = -1;
     int flip = 0;
@@ -1569,6 +1591,14 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
                 if (c->fq_dedup) c->dup_flags = (const uint8_t*)c->fq_dupflags.p;
             }
             struct FlagsBack { fp_ctx* c; const uint8_t* f; ~FlagsBack() { c->dup_flags = f; } } flags_back{c, saved_flags};
+            const uint8_t* rtext[2] = {(const uint8_t*)c->fqh_text[0].p + rstart[0], sides == 2 ? (const uint8_t*)c->fqh_text[1].p + rstart[1] : nullptr};
+            if (il_in) rtext[1] = rtext[0];                       /* both mates' records point into the one text */
+            if (c->fq_ix_on) {                                    /* filterByIndex, after the duplicate check (:404-410) */
+                if ((rc = index_flags_launch(c, rtext[0], (const fq_rec*)c->fqh_recs[0].p, rtext[1], (const fq_rec*)c->fqh_recs[1].p, n,
+                                             (uint8_t*)c->fq_ixflags.p, st))) return rc;
+                c->ix_flags = (const uint8_t*)c->fq_ixflags.p;    /* for this launch only (a caller's pointer was refused above) */
+            }
+            struct IndexBack { fp_ctx* c; ~IndexBack() { c->ix_flags = nullptr; } } index_back{c};
             if (sides == 2) {
                 c->ovx = ovx ? (fp_overlapped_result*)c->fqh_ovx.p : nullptr;   /* for this launch only (the sink was refused above) */
                 struct SinkBack { fp_ctx* c; ~SinkBack() { c->ovx = nullptr; } } sink_back{c};
@@ -1577,8 +1607,6 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
             } else rc = launch_chain(c, &b, (fp_read_result*)c->fqh_res[0].p, nullptr, nullptr, nullptr, 0, nullptr, st);
             if (rc) return rc;
             CK(cudaEventSynchronize(c->fq_ev_out[flip]));        /* the output buffers of two rounds ago have gone down */
-            const uint8_t* rtext[2] = {(const uint8_t*)c->fqh_text[0].p + rstart[0], sides == 2 ? (const uint8_t*)c->fqh_text[1].p + rstart[1] : nullptr};
-            if (il_in) rtext[1] = rtext[0];                       /* both mates' records point into the one text */
             for (int s = 0; s < NOUT; s++) {
                 if (!outs[s]) continue;                           /* caller does not want this stream's text */
                 fp_ctx::Buf& ob = c->fqh_outbuf[flip][s];
@@ -1739,6 +1767,76 @@ extern "C" int fp_dup_check(fp_ctx* c, const fp_batch* b, int32_t accuracy_level
 extern "C" int fp_set_dup_flags(fp_ctx* c, const uint8_t* d_is_dup) {
     if (!c) return set_err(FP_E_INVAL, "null argument");
     c->dup_flags = d_is_dup;
+    return FP_OK;
+}
+
+extern "C" int fp_set_index_flags(fp_ctx* c, const uint8_t* d_flags) {
+    if (!c) return set_err(FP_E_INVAL, "null argument");
+    c->ix_flags = d_flags;
+    return FP_OK;
+}
+
+/* Options::makeListFromFileByLine keeps A/C/G/T lines only (options.cpp:484-510); the lists go up packed as fq_index_list describes */
+extern "C" int fp_fastq_set_index_filter(fp_ctx* c, const char* const* list1, int64_t n1, const char* const* list2, int64_t n2, int32_t threshold) {
+    if (!c) return set_err(FP_E_INVAL, "null argument");
+    if (n1 < 0 || n2 < 0 || (n1 > 0 && !list1) || (n2 > 0 && !list2)) return set_err(FP_E_INVAL, "null argument");
+    if (n1 >= ((int64_t)1 << 31) || n2 >= ((int64_t)1 << 31)) return set_err(FP_E_TOOLARGE, "barcode list longer than 2^31");
+    const char* const* lists[2] = {list1, list2};
+    const int64_t ns[2] = {n1, n2};
+    std::vector<uint32_t> words[2];
+    std::vector<uint16_t> lens[2];
+    int W[2] = {1, 1};
+    for (int k = 0; k < 2; k++) {
+        for (int64_t b = 0; b < ns[k]; b++) {
+            const char* bc = lists[k][b];
+            if (!bc) return set_err(FP_E_INVAL, "null barcode");
+            const size_t len = strlen(bc);
+            if (len > FP_INDEX_MAX_BARCODE) return set_err(FP_E_INVAL, "barcode longer than FP_INDEX_MAX_BARCODE bytes");
+            for (size_t t = 0; t < len; t++)
+                if (bc[t] != 'A' && bc[t] != 'C' && bc[t] != 'G' && bc[t] != 'T') return set_err(FP_E_INVAL, "a barcode can only contain A/T/C/G");
+            W[k] = std::max(W[k], (int)((len + 31) / 32));
+        }
+        const int64_t n = ns[k];
+        words[k].assign((size_t)2 * W[k] * n, 0u);
+        lens[k].resize((size_t)n);
+        for (int64_t b = 0; b < n; b++) {
+            const char* bc = lists[k][b];
+            const size_t len = strlen(bc);
+            lens[k][b] = (uint16_t)len;
+            for (size_t t = 0; t < len; t++) {
+                const unsigned code = bc[t] == 'C' ? 1u : bc[t] == 'G' ? 2u : bc[t] == 'T' ? 3u : 0u;
+                const size_t w = t / 32;
+                words[k][w * n + b] |= (code & 1u) << (t % 32);
+                words[k][((size_t)W[k] + w) * n + b] |= (code >> 1) << (t % 32);
+            }
+        }
+    }
+    CK(cudaSetDevice(c->device));
+    CK(cudaDeviceSynchronize());                                   /* nothing may still read the old lists */
+    int rc;
+    for (int k = 0; k < 2; k++) {
+        if ((rc = fq_ensure(c->fq_ix_words[k], words[k].size() * 4 + 4))) return rc;
+        if ((rc = fq_ensure(c->fq_ix_lens[k], lens[k].size() * 2 + 2))) return rc;
+    }
+    for (int k = 0; k < 2; k++) {
+        if (!words[k].empty()) CK(cudaMemcpy(c->fq_ix_words[k].p, words[k].data(), words[k].size() * 4, cudaMemcpyHostToDevice));
+        if (!lens[k].empty()) CK(cudaMemcpy(c->fq_ix_lens[k].p, lens[k].data(), lens[k].size() * 2, cudaMemcpyHostToDevice));
+        c->fq_ix_n[k] = (int)ns[k]; c->fq_ix_w[k] = W[k];
+    }
+    c->fq_ix_thr = threshold;
+    c->fq_ix_on = n1 + n2 > 0;                                     /* initIndexFiltering: on when a list is non-empty (options.cpp:476-480) */
+    return FP_OK;
+}
+
+extern "C" int fp_fastq_index_flags(fp_ctx* c, const uint8_t* d_text1, const fp_fastq_rec* d_recs1, const uint8_t* d_text2, const fp_fastq_rec* d_recs2,
+                                    int64_t n, uint8_t* d_flags) {
+    if (!c) return set_err(FP_E_INVAL, "null argument");
+    if (n <= 0) return FP_OK;
+    if (!d_text1 || !d_recs1 || !d_flags || (c->p.paired && (!d_text2 || !d_recs2))) return set_err(FP_E_INVAL, "null argument");
+    CK(cudaSetDevice(c->device));
+    int rc = index_flags_launch(c, d_text1, (const fq_rec*)d_recs1, d_text2, (const fq_rec*)d_recs2, n, d_flags, c->stream[0]);
+    if (rc) return rc;
+    CK(cudaStreamSynchronize(c->stream[0]));
     return FP_OK;
 }
 

@@ -1228,7 +1228,14 @@ __device__ __forceinline__ fp_read_result t_make_result(const TRead& r, int verd
     if (r.null) { o.front = 0; o.len = 0; flags |= FP_F_DROPPED; }
     else { o.front = (uint16_t)r.front; o.len = (uint16_t)r.len; }
     o.verdict = (uint8_t)verdict; o.flags = (uint8_t)flags; o.adapter_pos = (int16_t)apos; o.adapter_len = (uint16_t)abases;
-    o.polyx_base = (uint8_t)pbase; o.pair_verdict = (uint8_t)pv; o.polyx_len = (uint16_t)plen; o.reserved = 0;
+    o.polyx_base = (uint8_t)pbase; o.pair_verdict = (uint8_t)pv; o.polyx_len = (uint16_t)plen; o.flags2 = 0;
+    return o;
+}
+/* the record of a read whose unit the index filter removed (seprocessor.cpp:220-224, peprocessor.cpp:404-410) */
+__device__ __forceinline__ fp_read_result t_index_filtered_result() {
+    fp_read_result o;
+    o.front = 0; o.len = 0; o.verdict = FP_FAIL_LENGTH; o.flags = FP_F_DROPPED; o.adapter_pos = 0; o.adapter_len = 0;
+    o.polyx_base = 255; o.pair_verdict = FP_FAIL_LENGTH; o.polyx_len = 0; o.flags2 = FP_F2_INDEX_FILTERED;
     return o;
 }
 
@@ -1795,7 +1802,11 @@ __global__ void __launch_bounds__(kChainThreads, 1) fp_chain2_kernel(const fp_la
                 TRead r1 = t_read(tile_seq[0] + rr * S, tile_planes + rr * PSTR, len0, clean);
                 int flags = 0, apos = 0, abases = 0, pbase = 255, plen = 0, result = FP_FAIL_LENGTH;
                 bool counted = false;
-                if (active) {
+                /* filterByIndex (:220-224): after the pre-filter Stats and the duplicate check, the unit leaves; its whole row is
+                   taken back out of the post-filter stats below (counted stays false) */
+                const bool ixf = active && a.ix_flags && a.ix_flags[gi];
+                if (ixf && lead) a.out1[gi] = t_index_filtered_result();
+                if (active && !ixf) {
                     tc_apply(r1, t_trim_and_cut(r1.seq(), r1.qual(), len0, c_p.trim_front1, c_p.trim_tail1, sub, GL, clean ? r1.pl() + 4 * PW : nullptr));   /* :235 */
                     if (!r1.null && c_p.polyg && !t_polyg_cannot_trim(r1, PW, c_p.polyg_min)) { const int nl = r1.clean ? t_trim_polyg_planes(r1.pl(), PW, r1.front, r1.len, c_p.polyg_min) : t_trim_polyg(r1.seq() + r1.front, r1.len, c_p.polyg_min); if (nl != r1.len) { r1.len = nl; flags |= FP_F_POLYG_TRIMMED; } }
                     bool dimer = false;
@@ -1845,7 +1856,16 @@ __global__ void __launch_bounds__(kChainThreads, 1) fp_chain2_kernel(const fp_la
                 fp_ov_result ov; ov.overlapped = 0; ov.has_gap = 0; ov.offset = 0; ov.overlap_len = 0; ov.diff = 0;
                 fp_ov_result ovA = ov;                    /* ovForAdapter */
                 bool both = false, need_correct = false;
-                if (active) {
+                /* filterByIndex (:404-410): the unit skips the chain but still reaches the CTA barriers of the correction round; its
+                   rows are taken back out of the post-filter stats below (counted stays false) */
+                const bool ixf = active && a.ix_flags && a.ix_flags[gi];
+                const bool run = active && !ixf;
+                if (ixf && lead) {
+                    a.out1[gi] = t_index_filtered_result(); a.out2[gi] = t_index_filtered_result();
+                    if (a.ov) a.ov[gi] = ov;
+                    if (a.ovx) { fp_overlapped_result ox; ox.overlapped = 0; ox._pad = 0; ox.offset = 0; ox.overlap_len = 0; ox.r1_len = 0; a.ovx[gi] = ox; }
+                }
+                if (run) {
                     tc_apply(r1, t_trim_and_cut(r1.seq(), r1.qual(), l1, c_p.trim_front1, c_p.trim_tail1, sub, GL, clean1 ? r1.pl() + 4 * PW : nullptr));   /* :425-426 */
                     tc_apply(r2, t_trim_and_cut(r2.seq(), r2.qual(), l2, c_p.trim_front2, c_p.trim_tail2, sub, GL, clean2 ? r2.pl() + 4 * PW : nullptr));
                     both = !r1.null && !r2.null;
@@ -1901,7 +1921,7 @@ __global__ void __launch_bounds__(kChainThreads, 1) fp_chain2_kernel(const fp_la
                 }
                 int res1 = FP_FAIL_LENGTH, res2 = FP_FAIL_LENGTH;
                 bool counted = false;
-                if (active) {
+                if (run) {
                     bool dimer = false;
                     if (need_correct) {
                         /* sequential path: pairs with bytes outside {A,C,G,T,N}, and what did not fit the work list (those positions still mismatch) */

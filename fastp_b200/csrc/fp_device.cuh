@@ -389,6 +389,7 @@ struct fp_launch_args {
     long long n_tiles;
     fp_smem_layout sl;
     fp_overlapped_result* ovx;       /* --overlapped_out (PE): the exact-overlap analysis of every unit (nullable) */
+    const uint8_t* ix_flags;         /* --filter_by_index1/2: units the index filter removes (nullable) */
 };
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {

@@ -445,6 +445,7 @@ __device__ __forceinline__ bool fq_passes(const fp_read_result& r) { return !(r.
 template <int SEL>
 __device__ __forceinline__ unsigned int fq_reject_plan(const fp_read_result& a, const fq_merge_args& M, long long i) {
     if (a.flags & FP_F_DUPLICATE) return 0u;                                             /* dedupOut (seprocessor.cpp:280, peprocessor.cpp:575) */
+    if (a.flags2 & FP_F2_INDEX_FILTERED) return 0u;                                      /* filterByIndex: the unit left before (seprocessor.cpp:220-224) */
     if (!M.res2) return SEL == FQ_SEL_FAILED && !fq_passes(a) ? fq_plan1(0, a.verdict) : 0u;        /* SE: seprocessor.cpp:281-289 */
     const fp_read_result& b = M.res2[i];
     if (M.merging && fq_unit_class(a, b, M.include_unmerged) != FQ_U_ORDINARY) return 0u; /* only the !mergeProcessed branch (:562) */
@@ -702,5 +703,95 @@ __global__ void __launch_bounds__(FQ_T) fq_encode_kernel(const uint8_t* text, co
         __syncthreads();
         if (threadIdx.x == FQ_T - 1) s_run = s_sz[FQ_T - 1] + sz;
         __syncthreads();
+    }
+}
+
+/* ---- index filter (--filter_by_index1 / --filter_by_index2; Read::firstIndex / lastIndex read.cpp:75-100, Filter::match filter.cpp:226-243) ----
+ * A barcode list is packed by the host into 2-bit planes, plane-major and barcode-minor so that the lanes of a warp, one barcode each,
+ * read consecutive words: words[(plane * W + w) * n + b] holds bases [32w, 32w + 32) of barcode b, bit t = base 32w + t, codes A0 C1 G2 T3
+ * (plane 0 the low bit).  W = words per plane of the longest barcode (>= 1).  The list is read through the read-only cache: its size is
+ * not limited by shared memory. */
+struct fq_index_list { const uint32_t* words; const uint16_t* lens; int n, W; };
+#define FQ_IX_WARPS 8
+#define FQ_IX_MAXW (FP_INDEX_MAX_BARCODE / 32)
+
+/* The index of one name by one warp: [s, e) of the name's bytes.  first = firstIndex, else lastIndex.  Walks the bytes from len-3 down
+ * 32 at a time; lane t looks at byte hi - t, so the lowest lane holding a separator is the first one met. */
+__device__ __forceinline__ void fq_index_span(const uint8_t* name, int len, bool first, int lane, int& s, int& e) {
+    s = e = 0;
+    if (len < 5) return;
+    int plus = len;                                            /* lowest '+' met so far: firstIndex ends before it */
+    for (int hi = len - 3; hi >= 0; hi -= 32) {
+        const int p = hi - lane;
+        const uint8_t c = p >= 0 ? name[p] : 0;
+        const unsigned mc = __ballot_sync(FULL_MASK, c == ':' || (!first && c == '+'));
+        const unsigned mp = __ballot_sync(FULL_MASK, c == '+');
+        if (mc) {
+            const int l = __ffs(mc) - 1;
+            const unsigned above = mp & ((1u << l) - 1u);       /* '+' bytes met before this separator */
+            if (first && above) plus = hi - (31 - __clz(above));
+            s = hi - l + 1;
+            e = first ? plus : len;
+            return;
+        }
+        if (mp) plus = hi - (31 - __clz(mp));
+    }
+}
+
+/* Whether any barcode of the list matches the index [s, e) of `name`; s_ix: this warp's 3 * FQ_IX_MAXW words of shared memory */
+__device__ __forceinline__ bool fq_index_match(const uint8_t* name, int s, int e, const fq_index_list& L, int threshold, uint32_t* s_ix, int lane) {
+    if (L.n == 0 || threshold < 0) return false;
+    const int ilen = e - s;
+    /* the index in the barcodes' planes, one word per step: lane t codes byte 32w + t, a ballot gathers the word; a byte outside
+       A/C/G/T clears its bit of the valid plane and so always counts as a mismatch */
+    for (int w = 0; w < L.W; w++) {
+        const int p = 32 * w + lane;
+        const uint8_t c = p < ilen ? name[s + p] : 0;
+        const unsigned code = c == 'C' ? 1u : c == 'G' ? 2u : c == 'T' ? 3u : 0u;
+        const bool ok = c == 'A' || c == 'C' || c == 'G' || c == 'T';
+        const unsigned lo = __ballot_sync(FULL_MASK, code & 1u), hi = __ballot_sync(FULL_MASK, code >> 1), va = __ballot_sync(FULL_MASK, ok);
+        if (lane == 0) { s_ix[w] = lo; s_ix[FQ_IX_MAXW + w] = hi; s_ix[2 * FQ_IX_MAXW + w] = va; }
+    }
+    __syncwarp();
+    bool hit = false;
+    for (int b0 = 0; b0 < L.n && !hit; b0 += 32) {
+        const int b = b0 + lane;
+        bool m = false;
+        if (b < L.n) {
+            const int common = min((int)__ldg(L.lens + b), ilen);
+            int diff = 0;
+            for (int w = 0; 32 * w < common && diff <= threshold; w++) {
+                const uint32_t blo = __ldg(L.words + (size_t)w * L.n + b), bhi = __ldg(L.words + (size_t)(L.W + w) * L.n + b);
+                uint32_t x = (s_ix[w] ^ blo) | (s_ix[FQ_IX_MAXW + w] ^ bhi) | ~s_ix[2 * FQ_IX_MAXW + w];
+                const int rest = common - 32 * w;
+                if (rest < 32) x &= (1u << rest) - 1u;
+                diff += __popc(x);
+            }
+            m = diff <= threshold;
+        }
+        hit = __any_sync(FULL_MASK, m);
+    }
+    __syncwarp();                                              /* s_ix is rewritten by the next call */
+    return hit;
+}
+
+/* flags[i] = whether Filter::filterByIndex removes unit i: one warp per unit.  text2 == NULL: single-end (list 1 only). */
+__global__ void __launch_bounds__(32 * FQ_IX_WARPS) fq_index_flags_kernel(const uint8_t* text1, const fq_rec* recs1, const uint8_t* text2, const fq_rec* recs2,
+                                                                          long long n, fq_index_list l1, fq_index_list l2, int threshold, uint8_t* flags) {
+    __shared__ uint32_t s_ix[FQ_IX_WARPS][3 * FQ_IX_MAXW];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    for (long long i = (long long)blockIdx.x * FQ_IX_WARPS + w; i < n; i += (long long)gridDim.x * FQ_IX_WARPS) {
+        const fq_rec r1 = recs1[i];
+        const uint8_t* name1 = text1 + r1.name_off;
+        int s, e;
+        fq_index_span(name1, (int)(r1.name_len & 0x0FFFFFFFu), true, lane, s, e);
+        bool f = fq_index_match(name1, s, e, l1, threshold, s_ix[w], lane);
+        if (!f && text2) {
+            const fq_rec r2 = recs2[i];
+            const uint8_t* name2 = text2 + r2.name_off;
+            fq_index_span(name2, (int)(r2.name_len & 0x0FFFFFFFu), false, lane, s, e);
+            f = fq_index_match(name2, s, e, l2, threshold, s_ix[w], lane);
+        }
+        if (lane == 0) flags[i] = f ? 1 : 0;
     }
 }

@@ -10,10 +10,42 @@
 #include <fstream>
 #include <iostream>
 #include <string>
+#include <sys/stat.h>
 #include <vector>
 #include "fastp_host.h"
 
 using namespace fastp_b200;
+
+/* Options::makeListFromFileByLine (src/options.cpp:484-510) after check_file_valid (src/util.h:185-194): one barcode per line read with
+   getline(line, 1000) -- a line of 1000 bytes or more ends the list there --, a trailing '\r' (or "\r\r") dropped only from lines of two
+   bytes or more, and any byte other than A/T/C/G ends the run.  Exit status and messages are the reference's. */
+static std::vector<std::string> loadBarcodes(const std::string& filename) {
+    struct stat st;
+    if (stat(filename.c_str(), &st) != 0) { std::cerr << "ERROR: file '" << filename << "' doesn't exist, quit now" << std::endl; exit(-1); }
+    if (S_ISDIR(st.st_mode)) { std::cerr << "ERROR: '" << filename << "' is a folder, not a file, quit now" << std::endl; exit(-1); }
+    std::vector<std::string> ret;
+    std::ifstream file(filename.c_str(), std::ifstream::in);
+    const int maxLine = 1000;
+    char line[maxLine];
+    std::cerr << "filter by index, loading " << filename << std::endl;
+    while (file.getline(line, maxLine)) {
+        const size_t got = strlen(line);             /* the line up to its first NUL byte, as the reference sees it */
+        if (got >= 2 && (line[got - 1] == '\n' || line[got - 1] == '\r')) {
+            line[got - 1] = '\0';
+            if (line[got - 2] == '\r') line[got - 2] = '\0';
+        }
+        const std::string bc(line);
+        for (char ch : bc)
+            if (ch != 'A' && ch != 'T' && ch != 'C' && ch != 'G') {
+                std::cerr << "ERROR: processing " << filename << ", each line should be one barcode, which can only contain A/T/C/G" << std::endl;
+                exit(-1);
+            }
+        std::cerr << bc << std::endl;
+        ret.push_back(bc);
+    }
+    std::cerr << std::endl;
+    return ret;
+}
 
 static Read* readRecord(std::istream& in) {          /* FastqReader::read src/fastqreader.cpp:309-368 (plain text only) */
     std::string name, seq, strand, qual;
@@ -26,7 +58,7 @@ static Read* readRecord(std::istream& in) {          /* FastqReader::read src/fa
 
 int main(int argc, char** argv) {
     Options opt;
-    std::string in1, in2, out1, out2, mergedOut, unpaired1, unpaired2, failedOut, overlappedOut, json;
+    std::string in1, in2, out1, out2, mergedOut, unpaired1, unpaired2, failedOut, overlappedOut, json, indexList1, indexList2;
     int packSize = 1 << 16, maxLen = 0;
     bool deviceFastq = false, phred64 = false;
     bool interleavedIn = false, fromStdin = false, toStdout = false;     /* src/main.cpp:194-196 */
@@ -41,6 +73,8 @@ int main(int argc, char** argv) {
         else if (a == "--unpaired1") unpaired1 = next(); else if (a == "--unpaired2") unpaired2 = next();
         else if (a == "--failed_out") failedOut = next();
         else if (a == "--overlapped_out") overlappedOut = next();
+        else if (a == "--filter_by_index1") indexList1 = next(); else if (a == "--filter_by_index2") indexList2 = next();
+        else if (a == "--filter_by_index_threshold") opt.indexFilter.threshold = atoi(next());
         else if (a == "-j" || a == "--json") json = next();
         else if (a == "-A" || a == "--disable_adapter_trimming") opt.adapter.enabled = false;
         else if (a == "-a" || a == "--adapter_sequence") { opt.adapter.sequence = next(); opt.adapter.hasSeqR1 = true; }
@@ -77,7 +111,7 @@ int main(int argc, char** argv) {
         else { fprintf(stderr, "unknown flag %s\n", a.c_str()); return 2; }
     }
     if (in1.empty() && fromStdin && in2.empty()) in1 = "/dev/stdin";    /* src/options.cpp:85-93 */
-    if (in1.empty()) { fprintf(stderr, "usage: fastp_gpu_cli -i R1.fq [-I R2.fq] [--interleaved_in] [--stdin] [--stdout] [-o out1.fq] [-O out2.fq] [-m --merged_out merged.fq] [--unpaired1 u1.fq] [--unpaired2 u2.fq] [--failed_out failed.fq] [--overlapped_out ov.fq] [-j summary.json] [fastp flags]\n"); return 2; }
+    if (in1.empty()) { fprintf(stderr, "usage: fastp_gpu_cli -i R1.fq [-I R2.fq] [--interleaved_in] [--stdin] [--stdout] [-o out1.fq] [-O out2.fq] [-m --merged_out merged.fq] [--unpaired1 u1.fq] [--unpaired2 u2.fq] [--failed_out failed.fq] [--overlapped_out ov.fq] [--filter_by_index1 list] [--filter_by_index2 list] [-j summary.json] [fastp flags]\n"); return 2; }
     if (!deviceFastq && (interleavedIn || fromStdin || toStdout)) { fprintf(stderr, "ERROR: --interleaved_in / --stdin / --stdout need --device_fastq\n"); return 2; }
     const bool stdinInput = in1 == "/dev/stdin";         /* read as it comes: nothing may open it twice */
     if (toStdout) {                                      /* src/options.cpp:101-110 */
@@ -89,6 +123,7 @@ int main(int argc, char** argv) {
         fprintf(stderr, "ERROR: --unpaired1 / --unpaired2 / --failed_out need --device_fastq\n"); return 2;
     }
     if (!deviceFastq && !overlappedOut.empty()) { fprintf(stderr, "ERROR: --overlapped_out needs --device_fastq\n"); return 2; }
+    if (!deviceFastq && !(indexList1.empty() && indexList2.empty())) { fprintf(stderr, "ERROR: --filter_by_index1 / --filter_by_index2 need --device_fastq\n"); return 2; }
     if (unpaired2.empty()) unpaired2 = unpaired1;       /* src/main.cpp:188-189 */
     auto fail = [](const char* msg) { fprintf(stderr, "ERROR: %s\n", msg); return 2; };
     if (opt.merge.enabled) {                            /* src/options.cpp:112-157 */
@@ -139,6 +174,9 @@ int main(int argc, char** argv) {
         if (failedOut == unpaired2) return fail("--failed_out and --unpaired2 shouldn't have same file name");
         if (opt.merge.enabled && failedOut == mergedOut) return fail("--failed_out and --merged_out shouldn't have same file name");
     }
+    if (!indexList1.empty()) opt.indexFilter.blacklist1 = loadBarcodes(indexList1);     /* Options::initIndexFiltering (src/options.cpp:462-481) */
+    if (!indexList2.empty()) opt.indexFilter.blacklist2 = loadBarcodes(indexList2);
+    opt.indexFilter.enabled = !(opt.indexFilter.blacklist1.empty() && opt.indexFilter.blacklist2.empty());
     /* the writers that exist (src/peprocessor.cpp:64-72): --unpaired2 has its own only when it names another file than --unpaired1 */
     const bool unpairedLeft = !unpaired1.empty(), unpairedRight = !unpaired2.empty() && unpaired2 != unpaired1;
     std::ifstream f1, f2;
@@ -190,6 +228,9 @@ int main(int argc, char** argv) {
         }
         if (evalDup || dedup) {                            /* accuracy level: 3 with --dedup, else 1, unless given (src/main.cpp:203-209) */
             if (!worker.setDedup(dupLevel ? dupLevel : (dedup ? 3 : 1), dedup)) { fprintf(stderr, "fastp_gpu_cli: duplicate filter: %s\n", fp_last_error()); return 1; }
+        }
+        if (opt.indexFilter.enabled && !worker.setIndexFilter(opt.indexFilter.blacklist1, opt.indexFilter.blacklist2, opt.indexFilter.threshold)) {
+            fprintf(stderr, "fastp_gpu_cli: index filter: %s\n", fp_last_error()); return 1;
         }
         /* text path: raw file chunks go to the device, which parses, filters and re-encodes them (fp_fastq_process_host);
            whatever a chunk's last, incomplete record (or the longer side of a pair) leaves over is carried into the next chunk */

@@ -50,6 +50,7 @@ struct Options {
     struct { bool enabled = true; int requiredLength = 15, maxLength = 0; } lengthFilter;
     struct { bool enabled = false; double threshold = 0.3; } complexityFilter;
     struct { bool enabled = false; int sampling = 20; } overRepAnalysis;           /* options.h:71-80 */
+    struct { bool enabled = false; std::vector<std::string> blacklist1, blacklist2; int threshold = 0; } indexFilter;   /* text path only */
     std::map<std::string, long> overRepSeqs1, overRepSeqs2;                        /* options.h:364-365, filled by the Evaluator pre-scan */
     int insertSizeMax = 512, overlapRequire = 30, overlapDiffLimit = 5, overlapDiffPercentLimit = 20;
     int seqLen1 = 151, seqLen2 = 151;
@@ -111,6 +112,13 @@ public:
     bool setInterleaved(bool in, bool out) {
         if (!mCtx || fp_fastq_set_interleaved(mCtx, in ? 1 : 0, out ? 1 : 0) != FP_OK) return false;
         mIlIn = in; mIlOut = out; return true;
+    }
+    /* text path: --filter_by_index1 / --filter_by_index2 (src/filter.cpp:209-243) with the lists Options::initIndexFiltering loaded */
+    bool setIndexFilter(const std::vector<std::string>& list1, const std::vector<std::string>& list2, int threshold) {
+        std::vector<const char*> l1, l2;
+        for (const std::string& b : list1) l1.push_back(b.c_str());
+        for (const std::string& b : list2) l2.push_back(b.c_str());
+        return mCtx && fp_fastq_set_index_filter(mCtx, l1.data(), (int64_t)l1.size(), l2.data(), (int64_t)l2.size(), threshold) == FP_OK;
     }
     bool dupTotals(long* total, long* dups) { int64_t t = 0, d = 0; if (!mCtx || fp_dup_totals(mCtx, &t, &d) != FP_OK) return false; *total = (long)t; *dups = (long)d; return true; }
     bool processFastqText(const char* text1, size_t n1, const char* text2, size_t n2, bool final, bool phred64,

@@ -163,6 +163,8 @@ typedef struct fp_batch {
 #define FP_F_ADAPTER_DIMER    0x20
 #define FP_F_MERGED           0x80  /* --merge: the pair overlapped and was merged (on both records); verdict = the merged read's */
 #define FP_F_DUPLICATE        0x40  /* dedupOut: flagged by the duplicate filter with --dedup on; not written, not in the post-filter stats (peprocessor.cpp:397-401,575) */
+/* flags2 */
+#define FP_F2_INDEX_FILTERED  0x01  /* --filter_by_index1/2 removed the unit (fp_set_index_flags): FP_F_DROPPED, pair_verdict FP_FAIL_LENGTH, on no stream */
 
 typedef struct fp_read_result {
     uint16_t front;        /* frontTrimmed: bases removed at the 5' end by trimAndCut          */
@@ -174,7 +176,7 @@ typedef struct fp_read_result {
     uint8_t  polyx_base;   /* 0..3 = A,T,C,G (ATCG_BASES common.h:25); 255 = none              */
     uint8_t  pair_verdict; /* code passed to addFilterResult: SE = verdict, PE = max(r1,r2)    */
     uint16_t polyx_len;    /* bases removed by trimPolyX                                       */
-    uint16_t reserved;
+    uint16_t flags2;       /* FP_F2_*; 0 unless the index filter is on                          */
 } fp_read_result;          /* 16 bytes */
 
 /* mirror of OverlapResult src/overlapanalysis.h:15-22 */
@@ -593,6 +595,33 @@ int  fp_dup_reset(fp_ctx* ctx);
  * `accuracy_level` on every round's decoded rows before the chain (0 = off) and drops duplicates from the output when `dedup` is set. */
 int  fp_set_dup_flags(fp_ctx* ctx, const uint8_t* d_is_dup);
 int  fp_fastq_set_dedup(fp_ctx* ctx, int32_t accuracy_level, int32_t dedup);
+
+/* --filter_by_index1 / --filter_by_index2 / --filter_by_index_threshold (src/filter.cpp:209-243, src/read.cpp:75-100).  The index of a read
+ * comes from its name line (the '@' included; a name shorter than 5 bytes has none): walking down from byte len-3 -- the last two bytes are
+ * never separators -- firstIndex is what follows the first ':' met, cut before the lowest '+' met on the way down; lastIndex is everything
+ * after the first ':' or '+' met.  No separator: the index is "".  A barcode matches an index when the two differ in at most `threshold`
+ * of the positions of the SHORTER one, so an empty index, an empty barcode, and a barcode that is a prefix of the index or the other way
+ * round all match whenever threshold >= 0; a negative threshold matches nothing.  Single-end: list 1 against firstIndex.  Paired-end:
+ * list 1 against read 1's firstIndex, then list 2 against read 2's lastIndex.  The reference removes such a unit after the pre-filter
+ * Stats (over-representation sampling included) and the duplicate filter, before everything else (src/seprocessor.cpp:209-224,
+ * src/peprocessor.cpp:392-410): no FilterResult counter, no insert size, no post-filter Stats, no output stream, --failed_out included.
+ * fp_set_index_flags: `d_flags` = DEVICE flags of the units of the next fp_process_se / _pe launches (non-zero = filtered), NULL switches it
+ * off.  Same contract as fp_set_dup_flags: indexed by unit of the LAUNCH, stays set until changed, and while it is set the host entry points
+ * (fp_process_*_host, _host_packed, _host_patches, fp_fastq_process_host*) return FP_E_INVAL.  A flagged unit keeps its pre-filter counters;
+ * its records are {front 0, len 0, verdict = pair_verdict = FP_FAIL_LENGTH, flags FP_F_DROPPED, polyx_base 255, flags2 FP_F2_INDEX_FILTERED},
+ * its overlap record and --overlapped_out analysis are zero, and its rows are left as they are.  A --dedup flag on the same unit is not
+ * consulted.
+ * fp_fastq_set_index_filter: the barcode lists of the text path (list1[n1], list2[n2], NUL-terminated, A/C/G/T only and at most
+ * FP_INDEX_MAX_BARCODE bytes each, else FP_E_INVAL and the filter is left as it was) and the threshold.  The filter is on when n1 + n2 > 0;
+ * (0, 0) switches it off.  Single-end: list 2 is accepted and not used, as in the reference.  Every round of fp_fastq_process_host, _merge and
+ * _outs then runs fp_fastq_index_flags on its decoded records after the duplicate filter and sets the flags for its launch.
+ * fp_fastq_index_flags: d_flags[i] for the records of a batch (all pointers DEVICE; text2 / recs2 NULL for single-end, the same text twice
+ * for interleaved input) under the ctx's lists; all 0 while the filter is off.  Synchronous. */
+#define FP_INDEX_MAX_BARCODE 1024
+int  fp_set_index_flags(fp_ctx* ctx, const uint8_t* d_flags);
+int  fp_fastq_set_index_filter(fp_ctx* ctx, const char* const* list1, int64_t n1, const char* const* list2, int64_t n2, int32_t threshold);
+int  fp_fastq_index_flags(fp_ctx* ctx, const uint8_t* d_text1, const fp_fastq_rec* d_recs1, const uint8_t* d_text2, const fp_fastq_rec* d_recs2,
+                          int64_t n, uint8_t* d_flags);
 
 /* --overlapped_out (src/peprocessor.cpp:488-495): after the adapter trimmers and before polyX, the reference runs the overlap analysis once
  * more with diffPercentLimit 0 on every pair whose two reads trimAndCut kept -- whatever the filters, the dimer check, --dedup or merging
