@@ -547,8 +547,12 @@ static int overrep_post_launch(fp_ctx* c, const fp_batch* b, const fp_read_resul
     return FP_OK;
 }
 
+/* what one launch reads beside its batch, indexed by the unit's index in the launch: --dedup flags, index-filter flags, and the
+   --overlapped_out sink the paired chain fills (each nullable) */
+struct chain_inputs { const uint8_t* is_dup; const uint8_t* ix_flags; fp_overlapped_result* ovx; };
+
 static int launch_chain(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_read_result* out2, fp_ov_result* ov,
-                        fp_patch* patches, uint32_t patch_cap, uint32_t* n_patches, cudaStream_t st) {
+                        fp_patch* patches, uint32_t patch_cap, uint32_t* n_patches, const chain_inputs& in, cudaStream_t st) {
     if (b->n == 0) return FP_OK;
     if (b->stride != c->stride) return set_err(FP_E_INVAL, "batch stride differs from the ctx stride");
     if (b->n > (int64_t)1 << 31) return set_err(FP_E_TOOLARGE, "batch larger than 2^31 (split it)");
@@ -558,9 +562,9 @@ static int launch_chain(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
     memset(&a, 0, sizeof(a));
     a.b = *b; a.out1 = out1; a.out2 = out2; a.ov = ov;
     a.sink.patches = patches; a.sink.cap = patches ? patch_cap : 0; a.sink.count = n_patches;
-    a.is_dup = c->dup_flags;
-    a.ovx = c->p.paired ? c->ovx : nullptr;
-    a.ix_flags = c->ix_flags;
+    a.is_dup = in.is_dup;
+    a.ovx = in.ovx;
+    a.ix_flags = in.ix_flags;
     a.events.events = c->ev_dev; a.events.cap = c->ev_dev ? c->ev_cap : 0; a.events.count = c->ev_count;
     a.counters = reinterpret_cast<unsigned long long*>(c->d_raw);
     a.n_tiles = (b->n + c->tile - 1) / c->tile;
@@ -632,7 +636,7 @@ extern "C" int fp_process_se(fp_ctx* c, const fp_batch* b, fp_read_result* out1,
     if (!c || !b || !out1) return set_err(FP_E_INVAL, "null argument");
     if (c->p.paired) return set_err(FP_E_INVAL, "ctx was created for paired-end data");
     CK(cudaSetDevice(c->device));
-    return launch_chain(c, b, out1, nullptr, nullptr, nullptr, 0, nullptr, stream ? (cudaStream_t)stream : c->stream[0]);
+    return launch_chain(c, b, out1, nullptr, nullptr, nullptr, 0, nullptr, {c->dup_flags, c->ix_flags, nullptr}, stream ? (cudaStream_t)stream : c->stream[0]);
 }
 
 extern "C" int fp_process_pe(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_read_result* out2, fp_ov_result* ov,
@@ -640,7 +644,7 @@ extern "C" int fp_process_pe(fp_ctx* c, const fp_batch* b, fp_read_result* out1,
     if (!c || !b || !out1 || !out2) return set_err(FP_E_INVAL, "null argument");
     if (!c->p.paired) return set_err(FP_E_INVAL, "ctx was created for single-end data");
     CK(cudaSetDevice(c->device));
-    return launch_chain(c, b, out1, out2, ov, patches, patch_cap, n_patches, stream ? (cudaStream_t)stream : c->stream[0]);
+    return launch_chain(c, b, out1, out2, ov, patches, patch_cap, n_patches, {c->dup_flags, c->ix_flags, c->ovx}, stream ? (cudaStream_t)stream : c->stream[0]);
 }
 
 /* ---------------- undo of a pass's base corrections / sharded over-representation sampling ---------------- */
@@ -1177,7 +1181,7 @@ static int process_host(fp_ctx* c, const fp_batch* b, fp_read_result* out1, fp_r
             else CK(cudaStreamWaitEvent(st, c->ovr_ev, 0));
         }
         rc = launch_chain(c, &db, c->d_out[slot][0].p, pe ? c->d_out[slot][1].p : nullptr, pe ? c->d_ov[slot].p : nullptr,
-                          pe ? c->d_patch[slot].p : nullptr, c->patch_cap, pe ? c->d_npatch[slot].p : nullptr, st);
+                          pe ? c->d_patch[slot].p : nullptr, c->patch_cap, pe ? c->d_npatch[slot].p : nullptr, chain_inputs{}, st);
         if (rc) return rc;
         if (c->p.overrep_enabled) CK(cudaEventRecord(c->ovr_ev, st));
         if (want_ev) CK(cudaMemcpyAsync(c->h_nev[slot].p, c->d_nev[slot].p, 4, cudaMemcpyDeviceToHost, st));
@@ -1364,13 +1368,49 @@ static int fastq_encode_impl(fp_ctx* c, const uint8_t* d_text, const fp_fastq_re
     return FP_OK;
 }
 
+/* one round's device arrays of both sides (index 0: read 1), the merging overlap results (ov) and the --overlapped_out analysis (ovx) */
+struct fq_round {
+    const uint8_t* text[2]; const fp_fastq_rec* recs[2]; const fp_read_result* res[2];
+    const uint8_t* seq[2]; const uint8_t* qual[2]; const uint16_t* len[2];
+    const fp_ov_result* ov; const fp_overlapped_result* ovx; int64_t n;
+};
+
+static_assert(FQ_SEL_UNPAIRED1 == FP_FQ_OUT_UNPAIRED1 && FQ_SEL_UNPAIRED2 == FP_FQ_OUT_UNPAIRED2 && FQ_SEL_FAILED == FP_FQ_OUT_FAILED,
+              "a reject stream's selector is its FP_FQ_OUT_* index");
+
+/* One output stream of a round: the only place that knows how each selector fills fq_merge_args.  side: the side FQ_SEL_PLAIN and
+   FQ_SEL_SIDE write (1: out2); writers: FP_FQ_W_* of the unpaired writers that exist (reject streams only). */
+static int fastq_encode_stream(fp_ctx* c, int sel, int side, const fq_round& R, int writers, uint8_t* d_out, int64_t out_cap, int64_t* out_bytes) {
+    fq_merge_args M{};
+    auto read2 = [&]() { M.text2 = R.text[1]; M.recs2 = reinterpret_cast<const fq_rec*>(R.recs[1]); M.res2 = R.res[1]; M.seq2 = R.seq[1]; M.qual2 = R.qual[1]; };
+    int s = 0;                                                    /* the side whose arrays are the primary ones */
+    switch (sel) {
+    case FQ_SEL_PLAIN: s = side; break;
+    case FQ_SEL_INTERLEAVED: read2(); break;
+    case FQ_SEL_MERGED: case FQ_SEL_SIDE:
+        M.ov = R.ov; M.include_unmerged = c->p.merge_include_unmerged ? 1 : 0;
+        if (side == 1) { s = 1; M.res2 = R.res[0]; }              /* side 2 is written, side 1 only gives its records */
+        else read2();
+        break;
+    case FQ_SEL_OVERLAPPED: M.res2 = R.res[1]; M.ovx = R.ovx; break;
+    default:                                                      /* the reject streams */
+        M.len1 = R.len[0]; M.writers = writers; M.merging = c->p.paired && c->p.merge_enabled; M.include_unmerged = c->p.merge_include_unmerged ? 1 : 0;
+        if (c->p.paired) { read2(); M.len2 = R.len[1]; }
+    }
+    static const decltype(&fastq_encode_impl<FQ_SEL_PLAIN>) encode[] = {   /* indexed by FQ_SEL_* */
+        fastq_encode_impl<FQ_SEL_PLAIN>, fastq_encode_impl<FQ_SEL_MERGED>, fastq_encode_impl<FQ_SEL_SIDE>, fastq_encode_impl<FQ_SEL_UNPAIRED1>,
+        fastq_encode_impl<FQ_SEL_UNPAIRED2>, fastq_encode_impl<FQ_SEL_FAILED>, fastq_encode_impl<FQ_SEL_INTERLEAVED>, fastq_encode_impl<FQ_SEL_OVERLAPPED>};
+    return encode[sel](c, R.text[s], R.recs[s], R.res[s], R.seq[s], R.qual[s], M, R.n, d_out, out_cap, out_bytes);
+}
+
 extern "C" int fp_fastq_encode(fp_ctx* c, const uint8_t* d_text, const fp_fastq_rec* d_recs, const fp_read_result* d_res,
                                const uint8_t* d_seq, const uint8_t* d_qual, int64_t n, uint8_t* d_out, int64_t out_cap, int64_t* out_bytes) {
     if (!c || !out_bytes) return set_err(FP_E_INVAL, "null argument");
     *out_bytes = 0;
     if (n <= 0) return FP_OK;
     if (!d_text || !d_recs || !d_res || !d_seq || !d_qual || (out_cap > 0 && !d_out)) return set_err(FP_E_INVAL, "null argument");
-    return fastq_encode_impl<FQ_SEL_PLAIN>(c, d_text, d_recs, d_res, d_seq, d_qual, fq_merge_args{}, n, d_out, out_cap, out_bytes);
+    const fq_round R = {{d_text}, {d_recs}, {d_res}, {d_seq}, {d_qual}, {}, nullptr, nullptr, n};
+    return fastq_encode_stream(c, FQ_SEL_PLAIN, 0, R, 0, d_out, out_cap, out_bytes);
 }
 
 extern "C" int fp_fastq_encode_interleaved(fp_ctx* c, const uint8_t* d_text1, const fp_fastq_rec* d_recs1, const uint8_t* d_text2, const fp_fastq_rec* d_recs2,
@@ -1384,9 +1424,8 @@ extern "C" int fp_fastq_encode_interleaved(fp_ctx* c, const uint8_t* d_text1, co
     if (n <= 0) return FP_OK;
     if (!d_text1 || !d_recs1 || !d_text2 || !d_recs2 || !d_res1 || !d_res2 || !d_seq1 || !d_qual1 || !d_seq2 || !d_qual2 || (out_cap > 0 && !d_out))
         return set_err(FP_E_INVAL, "null argument");
-    fq_merge_args M{};
-    M.text2 = d_text2; M.recs2 = reinterpret_cast<const fq_rec*>(d_recs2); M.res2 = d_res2; M.seq2 = d_seq2; M.qual2 = d_qual2;
-    return fastq_encode_impl<FQ_SEL_INTERLEAVED>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
+    const fq_round R = {{d_text1, d_text2}, {d_recs1, d_recs2}, {d_res1, d_res2}, {d_seq1, d_seq2}, {d_qual1, d_qual2}, {}, nullptr, nullptr, n};
+    return fastq_encode_stream(c, FQ_SEL_INTERLEAVED, 0, R, 0, d_out, out_cap, out_bytes);
 }
 
 extern "C" int fp_fastq_encode_merge(fp_ctx* c, int32_t which, const uint8_t* d_text1, const fp_fastq_rec* d_recs1, const uint8_t* d_text2, const fp_fastq_rec* d_recs2,
@@ -1401,15 +1440,8 @@ extern "C" int fp_fastq_encode_merge(fp_ctx* c, int32_t which, const uint8_t* d_
     if (n <= 0) return FP_OK;
     if (!d_text1 || !d_recs1 || !d_text2 || !d_recs2 || !d_res1 || !d_res2 || !d_ov || !d_seq1 || !d_qual1 || !d_seq2 || !d_qual2 || (out_cap > 0 && !d_out))
         return set_err(FP_E_INVAL, "null argument");
-    fq_merge_args M{};
-    M.ov = d_ov; M.include_unmerged = c->p.merge_include_unmerged ? 1 : 0;
-    if (which == FP_FQ_OUT_R2) {                                  /* side 2 is written, side 1 only gives its records */
-        M.res2 = d_res1;
-        return fastq_encode_impl<FQ_SEL_SIDE>(c, d_text2, d_recs2, d_res2, d_seq2, d_qual2, M, n, d_out, out_cap, out_bytes);
-    }
-    M.text2 = d_text2; M.recs2 = reinterpret_cast<const fq_rec*>(d_recs2); M.res2 = d_res2; M.seq2 = d_seq2; M.qual2 = d_qual2;
-    if (which == FP_FQ_OUT_R1) return fastq_encode_impl<FQ_SEL_SIDE>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
-    return fastq_encode_impl<FQ_SEL_MERGED>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
+    const fq_round R = {{d_text1, d_text2}, {d_recs1, d_recs2}, {d_res1, d_res2}, {d_seq1, d_seq2}, {d_qual1, d_qual2}, {}, d_ov, nullptr, n};
+    return fastq_encode_stream(c, which == FP_FQ_OUT_MERGED ? FQ_SEL_MERGED : FQ_SEL_SIDE, which == FP_FQ_OUT_R2 ? 1 : 0, R, 0, d_out, out_cap, out_bytes);
 }
 
 extern "C" int fp_fastq_encode_overlapped(fp_ctx* c, const uint8_t* d_text1, const fp_fastq_rec* d_recs1, const fp_read_result* d_res1,
@@ -1420,9 +1452,8 @@ extern "C" int fp_fastq_encode_overlapped(fp_ctx* c, const uint8_t* d_text1, con
     if (!c->p.paired) return set_err(FP_E_INVAL, "ctx was created for single-end data: --overlapped_out needs pairs");
     if (n <= 0) return FP_OK;
     if (!d_text1 || !d_recs1 || !d_res1 || !d_res2 || !d_ovx || !d_seq1 || !d_qual1 || (out_cap > 0 && !d_out)) return set_err(FP_E_INVAL, "null argument");
-    fq_merge_args M{};
-    M.res2 = d_res2; M.ovx = d_ovx;
-    return fastq_encode_impl<FQ_SEL_OVERLAPPED>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
+    const fq_round R = {{d_text1}, {d_recs1}, {d_res1, d_res2}, {d_seq1}, {d_qual1}, {}, nullptr, d_ovx, n};
+    return fastq_encode_stream(c, FQ_SEL_OVERLAPPED, 0, R, 0, d_out, out_cap, out_bytes);
 }
 
 /* the argument rules of fp_fastq_encode_rejects and fp_fastq_process_host_outs (options.cpp:136-143, :222-229) */
@@ -1451,12 +1482,8 @@ extern "C" int fp_fastq_encode_rejects(fp_ctx* c, int32_t which, int32_t writers
     if (!d_text1 || !d_recs1 || !d_res1 || !d_seq1 || !d_qual1 || !d_len1 || (out_cap > 0 && !d_out) ||
         (pe && (!d_text2 || !d_recs2 || !d_res2 || !d_seq2 || !d_qual2 || !d_len2)))
         return set_err(FP_E_INVAL, "null argument");
-    fq_merge_args M{};
-    M.len1 = d_len1; M.writers = writers; M.merging = pe && c->p.merge_enabled; M.include_unmerged = c->p.merge_include_unmerged ? 1 : 0;
-    if (pe) { M.text2 = d_text2; M.recs2 = reinterpret_cast<const fq_rec*>(d_recs2); M.res2 = d_res2; M.seq2 = d_seq2; M.qual2 = d_qual2; M.len2 = d_len2; }
-    if (which == FP_FQ_OUT_UNPAIRED1) return fastq_encode_impl<FQ_SEL_UNPAIRED1>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
-    if (which == FP_FQ_OUT_UNPAIRED2) return fastq_encode_impl<FQ_SEL_UNPAIRED2>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
-    return fastq_encode_impl<FQ_SEL_FAILED>(c, d_text1, d_recs1, d_res1, d_seq1, d_qual1, M, n, d_out, out_cap, out_bytes);
+    const fq_round R = {{d_text1, d_text2}, {d_recs1, d_recs2}, {d_res1, d_res2}, {d_seq1, d_seq2}, {d_qual1, d_qual2}, {d_len1, d_len2}, nullptr, nullptr, n};
+    return fastq_encode_stream(c, which, 0, R, writers, d_out, out_cap, out_bytes);
 }
 
 /* Filter::filterByIndex over a batch of decoded records (fq_index_flags_kernel), enqueued on st */
@@ -1584,62 +1611,45 @@ static int fastq_process_host_impl(fp_ctx* c, const uint8_t* text1, int64_t nbyt
             b.n = n; b.stride = c->stride;
             b.seq1 = (uint8_t*)c->fqh_seq[0].p; b.qual1 = (uint8_t*)c->fqh_qual[0].p; b.len1 = (uint16_t*)c->fqh_len[0].p;
             if (sides == 2) { b.seq2 = (uint8_t*)c->fqh_seq[1].p; b.qual2 = (uint8_t*)c->fqh_qual[1].p; b.len2 = (uint16_t*)c->fqh_len[1].p; }
-            const uint8_t* saved_flags = c->dup_flags;
+            chain_inputs in{};                                    /* this launch's own flags and sink (a caller's were refused above) */
             if (c->fq_dup_level > 0) {                            /* Duplicate::checkRead / checkPair on the reads as read, before the chain (:397-401) */
                 if ((rc = fq_ensure(c->fq_dupflags, (size_t)cap))) return rc;
                 if ((rc = fp_dup_check(c, &b, c->fq_dup_level, (uint8_t*)c->fq_dupflags.p, st))) return rc;
-                if (c->fq_dedup) c->dup_flags = (const uint8_t*)c->fq_dupflags.p;
+                if (c->fq_dedup) in.is_dup = (const uint8_t*)c->fq_dupflags.p;
             }
-            struct FlagsBack { fp_ctx* c; const uint8_t* f; ~FlagsBack() { c->dup_flags = f; } } flags_back{c, saved_flags};
             const uint8_t* rtext[2] = {(const uint8_t*)c->fqh_text[0].p + rstart[0], sides == 2 ? (const uint8_t*)c->fqh_text[1].p + rstart[1] : nullptr};
             if (il_in) rtext[1] = rtext[0];                       /* both mates' records point into the one text */
             if (c->fq_ix_on) {                                    /* filterByIndex, after the duplicate check (:404-410) */
                 if ((rc = index_flags_launch(c, rtext[0], (const fq_rec*)c->fqh_recs[0].p, rtext[1], (const fq_rec*)c->fqh_recs[1].p, n,
                                              (uint8_t*)c->fq_ixflags.p, st))) return rc;
-                c->ix_flags = (const uint8_t*)c->fq_ixflags.p;    /* for this launch only (a caller's pointer was refused above) */
+                in.ix_flags = (const uint8_t*)c->fq_ixflags.p;
             }
-            struct IndexBack { fp_ctx* c; ~IndexBack() { c->ix_flags = nullptr; } } index_back{c};
-            if (sides == 2) {
-                c->ovx = ovx ? (fp_overlapped_result*)c->fqh_ovx.p : nullptr;   /* for this launch only (the sink was refused above) */
-                struct SinkBack { fp_ctx* c; ~SinkBack() { c->ovx = nullptr; } } sink_back{c};
-                rc = launch_chain(c, &b, (fp_read_result*)c->fqh_res[0].p, (fp_read_result*)c->fqh_res[1].p, merging ? (fp_ov_result*)c->fqh_ov.p : nullptr,
-                                  nullptr, 0, nullptr, st);
-            } else rc = launch_chain(c, &b, (fp_read_result*)c->fqh_res[0].p, nullptr, nullptr, nullptr, 0, nullptr, st);
+            if (ovx) in.ovx = (fp_overlapped_result*)c->fqh_ovx.p;
+            rc = launch_chain(c, &b, (fp_read_result*)c->fqh_res[0].p, sides == 2 ? (fp_read_result*)c->fqh_res[1].p : nullptr,
+                              merging ? (fp_ov_result*)c->fqh_ov.p : nullptr, nullptr, 0, nullptr, in, st);
             if (rc) return rc;
+            const fq_round R = {{rtext[0], rtext[1]}, {(const fp_fastq_rec*)c->fqh_recs[0].p, (const fp_fastq_rec*)c->fqh_recs[1].p},
+                                {(const fp_read_result*)c->fqh_res[0].p, (const fp_read_result*)c->fqh_res[1].p},
+                                {(const uint8_t*)c->fqh_seq[0].p, (const uint8_t*)c->fqh_seq[1].p}, {(const uint8_t*)c->fqh_qual[0].p, (const uint8_t*)c->fqh_qual[1].p},
+                                {(const uint16_t*)c->fqh_len[0].p, (const uint16_t*)c->fqh_len[1].p},
+                                (const fp_ov_result*)c->fqh_ov.p, (const fp_overlapped_result*)c->fqh_ovx.p, n};
             CK(cudaEventSynchronize(c->fq_ev_out[flip]));        /* the output buffers of two rounds ago have gone down */
             for (int s = 0; s < NOUT; s++) {
                 if (!outs[s]) continue;                           /* caller does not want this stream's text */
+                /* the entry points and the checks above leave the encoder nothing to refuse: a merged buffer comes only with merging, interleaved
+                   output never merges and has no out2, reject buffers only where fastq_rejects_check allows them, OVX only on a paired ctx */
+                const int sel = s == OVX ? FQ_SEL_OVERLAPPED : s >= FP_FQ_OUT_UNPAIRED1 ? s : il_out ? FQ_SEL_INTERLEAVED
+                              : merging ? (s == FP_FQ_OUT_MERGED ? FQ_SEL_MERGED : FQ_SEL_SIDE) : FQ_SEL_PLAIN;
                 fp_ctx::Buf& ob = c->fqh_outbuf[flip][s];
                 const int64_t room = std::max<int64_t>(ocap[s] - obytes[s], 0);
-                /* per unit: one record of a side; on the merged stream one read of up to two rows, or two records; on the failed stream two
-                   tagged records */
-                const bool two = s == FP_FQ_OUT_MERGED || s == FP_FQ_OUT_FAILED || (il_out && s == FP_FQ_OUT_R1);
+                /* per unit: one record of a side; on the merged stream one read of up to two rows, or two records; on the interleaved stream two
+                   records; on the failed stream two tagged records */
+                const bool two = sel == FQ_SEL_MERGED || sel == FQ_SEL_INTERLEAVED || sel == FQ_SEL_FAILED;
                 int64_t want = std::min<int64_t>(room, n * (int64_t)(two ? 4 * c->stride + 512 : 2 * c->stride + 256));
                 int64_t total = 0;
-                const fp_fastq_rec* recs[2] = {(const fp_fastq_rec*)c->fqh_recs[0].p, (const fp_fastq_rec*)c->fqh_recs[1].p};
-                const fp_read_result* res[2] = {(const fp_read_result*)c->fqh_res[0].p, (const fp_read_result*)c->fqh_res[1].p};
-                const uint8_t* seq[2] = {(const uint8_t*)c->fqh_seq[0].p, (const uint8_t*)c->fqh_seq[1].p};
-                const uint8_t* qual[2] = {(const uint8_t*)c->fqh_qual[0].p, (const uint8_t*)c->fqh_qual[1].p};
                 for (int attempt = 0; attempt < 2; attempt++) {   /* names longer than the estimate: encode again into a buffer of the exact size */
                     if ((rc = fq_ensure(ob, (size_t)want + 64))) return rc;
-                    if (s == OVX)
-                        rc = fp_fastq_encode_overlapped(c, rtext[0], recs[0], res[0], res[1], (const fp_overlapped_result*)c->fqh_ovx.p, seq[0], qual[0],
-                                                        n, (uint8_t*)ob.p, want, &total);
-                    else if (s >= FP_FQ_OUT_UNPAIRED1)
-                        rc = fp_fastq_encode_rejects(c, s, writers, rtext[0], recs[0], rtext[1], recs[1], res[0], res[1], seq[0], qual[0],
-                                                     (const uint16_t*)c->fqh_len[0].p, seq[1], qual[1], (const uint16_t*)c->fqh_len[1].p,
-                                                     n, (uint8_t*)ob.p, want, &total);
-                    else if (il_out)                              /* s == FP_FQ_OUT_R1: an out2 buffer was refused above */
-                        rc = fp_fastq_encode_interleaved(c, rtext[0], recs[0], rtext[1], recs[1], res[0], res[1], seq[0], qual[0], seq[1], qual[1],
-                                                         n, (uint8_t*)ob.p, want, &total);
-                    else if (merging)
-                        rc = fp_fastq_encode_merge(c, s, rtext[0], recs[0], rtext[1], recs[1], res[0], res[1], (const fp_ov_result*)c->fqh_ov.p,
-                                                   seq[0], qual[0], seq[1], qual[1], n, (uint8_t*)ob.p, want, &total);
-                    else {
-                        const int side = s == FP_FQ_OUT_R2 ? 1 : 0;
-                        rc = fp_fastq_encode(c, rtext[side], recs[side], res[side], seq[side], qual[side], n, (uint8_t*)ob.p, want, &total);
-                    }
-                    if (rc) return rc;
+                    if ((rc = fastq_encode_stream(c, sel, s == FP_FQ_OUT_R2 ? 1 : 0, R, writers, (uint8_t*)ob.p, want, &total))) return rc;
                     if (total <= want) break;
                     if (total > room) return set_err(FP_E_TOOLARGE, "output buffer too small for the encoded FASTQ text");
                     want = total;

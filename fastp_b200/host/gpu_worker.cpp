@@ -174,9 +174,7 @@ bool GpuChainWorker::processPairEnd(ReadPack* leftPack, ReadPack* rightPack, std
 }
 
 bool GpuChainWorker::processFastqText(const char* text1, size_t n1, const char* text2, size_t n2, bool final, bool phred64,
-                                      std::string* outstr1, std::string* outstr2, size_t* consumed1, size_t* consumed2, long* units,
-                                      std::string* merged, std::string* unpaired1, std::string* unpaired2, std::string* failed,
-                                      std::string* overlapped) {
+                                      std::string* const outs[FQ_TEXT_OUTS], size_t* consumed1, size_t* consumed2, long* units) {
     const bool paired = mParams.paired != 0, merging = paired && mParams.merge_enabled;
     const bool ilIn = paired && mIlIn, ilOut = paired && mIlOut;
     if (ilIn) n2 = 0;                                           /* both mates are in text1 */
@@ -187,28 +185,26 @@ bool GpuChainWorker::processFastqText(const char* text1, size_t n1, const char* 
     const size_t side2 = ilIn ? n1 : n2;                        /* the text that holds read 2 */
     /* what each stream can hold at most: a side's reads (both sides' when interleaved); on the merged stream everything both inputs hold, each
        merged read with its name suffix (one per pair, i.e. per 8 lines at least); on unpaired1 reads of either side; on the failed stream
-       reads of either side, each with a tag of up to 24 bytes (a record takes 6 bytes at least) */
-    std::string* want[FP_FQ_OUTS] = {merging ? merged : nullptr, outstr1, paired && !ilOut ? outstr2 : nullptr, paired ? unpaired1 : nullptr,
-                                     paired ? unpaired2 : nullptr, failed};
-    const size_t cap[FP_FQ_OUTS] = {n1 + n2 + (n1 / 8 + 1) * 40 + 64, (ilOut ? both : n1) + 64, side2 + 64, both + 64, side2 + 64,
-                                    both + (both / 6 + 2) * 24 + 64};
-    uint8_t* outs[FP_FQ_OUTS]; int64_t caps[FP_FQ_OUTS], ob[FP_FQ_OUTS];
-    for (int s = 0; s < FP_FQ_OUTS; s++) {
+       reads of either side, each with a tag of up to 24 bytes (a record takes 6 bytes at least); on --overlapped_out at most one record of
+       read 1 per pair, never longer than read 1's input record */
+    std::string* want[FQ_TEXT_OUTS] = {merging ? outs[FP_FQ_OUT_MERGED] : nullptr, outs[FP_FQ_OUT_R1], paired && !ilOut ? outs[FP_FQ_OUT_R2] : nullptr,
+                                       paired ? outs[FP_FQ_OUT_UNPAIRED1] : nullptr, paired ? outs[FP_FQ_OUT_UNPAIRED2] : nullptr, outs[FP_FQ_OUT_FAILED],
+                                       paired ? outs[FQ_OUT_OVERLAPPED] : nullptr};
+    const size_t cap[FQ_TEXT_OUTS] = {n1 + n2 + (n1 / 8 + 1) * 40 + 64, (ilOut ? both : n1) + 64, side2 + 64, both + 64, side2 + 64,
+                                      both + (both / 6 + 2) * 24 + 64, n1 + 64};
+    uint8_t* bufs[FQ_TEXT_OUTS]; int64_t caps[FQ_TEXT_OUTS], ob[FQ_TEXT_OUTS] = {0};
+    for (int s = 0; s < FQ_TEXT_OUTS; s++) {
         if (want[s]) mTextOut[s].resize(cap[s]);
-        outs[s] = want[s] ? mTextOut[s].data() : nullptr;
+        bufs[s] = want[s] ? mTextOut[s].data() : nullptr;
         caps[s] = want[s] ? (int64_t)cap[s] : 0;
     }
-    /* --overlapped_out: at most one record of read 1 per pair, never longer than read 1's input record */
-    int64_t obOv = 0;
-    if (paired && overlapped) {
-        mTextOut[FP_FQ_OUTS].resize(n1 + 64);
-        if (fp_fastq_set_overlapped_out(mCtx, mTextOut[FP_FQ_OUTS].data(), (int64_t)(n1 + 64), &obOv) != FP_OK) { mError = fp_last_error(); return false; }
-    }
-    const int rc = fp_fastq_process_host_outs(mCtx, t1, (int64_t)n1, t2, paired ? (int64_t)n2 : 0, final ? 1 : 0, phred64 ? 1 : 0, outs, caps, ob,
+    /* --overlapped_out is not one of the C-ABI's FP_FQ_OUTS streams: its buffer is attached to the ctx for this call */
+    const bool ov = want[FQ_OUT_OVERLAPPED] != nullptr;
+    if (ov && fp_fastq_set_overlapped_out(mCtx, bufs[FQ_OUT_OVERLAPPED], caps[FQ_OUT_OVERLAPPED], &ob[FQ_OUT_OVERLAPPED]) != FP_OK) { mError = fp_last_error(); return false; }
+    const int rc = fp_fastq_process_host_outs(mCtx, t1, (int64_t)n1, t2, paired ? (int64_t)n2 : 0, final ? 1 : 0, phred64 ? 1 : 0, bufs, caps, ob,
                                               &nu, &c1, paired ? &c2 : nullptr, &i1, paired ? &i2 : nullptr);
-    if (paired && overlapped) fp_fastq_set_overlapped_out(mCtx, nullptr, 0, nullptr);
+    if (ov) fp_fastq_set_overlapped_out(mCtx, nullptr, 0, nullptr);
     if (rc != FP_OK) { mError = fp_last_error(); return false; }
-    if (paired && overlapped) overlapped->append(reinterpret_cast<const char*>(mTextOut[FP_FQ_OUTS].data()), (size_t)obOv);
     if (i1.error == FP_FQ_ERR_STRIDE || (paired && i2.error == FP_FQ_ERR_STRIDE)) { mError = "a read is longer than the row stride (raise --max_read_len)"; return false; }
     if (i1.error != FP_FQ_OK || (paired && i2.error != FP_FQ_OK)) {
         const fp_fastq_info& bad = i1.error != FP_FQ_OK ? i1 : i2;
@@ -216,7 +212,7 @@ bool GpuChainWorker::processFastqText(const char* text1, size_t n1, const char* 
                 bad.error == FP_FQ_ERR_STRAND ? "Expected '+'" : "ERROR: sequence and quality have different length:", (long long)bad.error_record, i1.error != FP_FQ_OK ? 1 : 2);
         mInputEnded = true;
     }
-    for (int s = 0; s < FP_FQ_OUTS; s++)
+    for (int s = 0; s < FQ_TEXT_OUTS; s++)
         if (want[s]) want[s]->append(reinterpret_cast<const char*>(mTextOut[s].data()), (size_t)ob[s]);
     if (consumed1) *consumed1 = (size_t)c1;
     if (consumed2) *consumed2 = (size_t)c2;
