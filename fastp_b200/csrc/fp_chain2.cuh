@@ -877,7 +877,10 @@ __device__ __forceinline__ int t_gap_scan(const uint8_t* ins, const uint8_t* nor
  * Random sequence fails at K = 8 nine times out of ten; what passes there is checked at 16, 24, 32 ... before the byte scan is paid. */
 __device__ __noinline__ bool gap_may_hit(unsigned long long D1, unsigned long long D2, int cmax) {
     const int amax = cmax / 8 - 1;                                        /* c/8 - 1 < 0 for every c < 8 */
-    const int kmax = min(cmax, 64) >> 3;
+    /* Bit 63 of scan 2's field compares read[64], which the 64-bit read field does not hold, with adapter[63]: only bits 0..62 are
+       true, so the walk stops at K = 56.  Every length c <= 63 is settled there; c = 64 (a 64-base adapter, a read of 65 and more)
+       is not, and goes to the byte scan unless B_56 already exceeds its allowance. */
+    const int kmax = min(cmax, 63) >> 3;
     /* B_K = popc(D2 & low(K)) + min_{0<=i<=K} S(i),  S(i) = popc(D1 & low(i)) - popc(D2 & low(i)): one walk over the bits, checked every 8 */
     int S = 0, M = 0, c2 = 0;
     #pragma unroll 1
@@ -891,7 +894,7 @@ __device__ __noinline__ bool gap_may_hit(unsigned long long D1, unsigned long lo
         if (v <= k - 1) return true;
         if (v > amax) return false;
     }
-    return false;
+    return cmax >= 64;
 }
 
 /* result of an adapter trimmer: 0 = not trimmed, else at_pack(new length, adapter position, adapter bases) -- one register

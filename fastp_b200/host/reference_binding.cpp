@@ -16,7 +16,8 @@
  * device's counter block to this worker's Stats / FilterResult objects, then the unchanged tail of the reference loop (output
  * strings, writers, recycling).  Merging mode (--merge / --include_unmerged, :519-560) runs on the device too: the merged Read is built
  * by the reference's own OverlapAnalysis::merge from the device's second overlap record.  Option sets the device path does not
- * cover (overlapped_out, UMI, over-representation analysis, reads longer than FP_MAX_STRIDE) are handed to the stock body.
+ * cover (overlapped_out, UMI, over-representation analysis, reads longer than FP_MAX_STRIDE, adapters past fp_ctx_create's limits) are
+ * handed to the stock body.
  */
 #include <algorithm>
 #include <cstdio>
@@ -131,8 +132,19 @@ GpuWorker* worker_for(const void* proc, Options* o, bool paired, int tid, int ne
     return w;
 }
 
+/* fp_ctx_create refuses adapters longer than FP_MAX_ADAPTER_LEN and more than FP_MAX_ADAPTERS fasta entries; the reference's loader
+   keeps both (src/options.cpp loadFastaAdapters drops only entries under 6 bases and duplicates), so such option sets run on the stock body */
+bool adapters_fit(Options* o) {
+    if ((o->adapter.hasSeqR1 && o->adapter.sequence.size() > FP_MAX_ADAPTER_LEN) || (o->adapter.hasSeqR2 && o->adapter.sequenceR2.size() > FP_MAX_ADAPTER_LEN))
+        return false;
+    if (!o->adapter.hasFasta) return true;
+    if (o->adapter.seqsInFasta.size() > FP_MAX_ADAPTERS) return false;
+    for (auto& s : o->adapter.seqsInFasta) if (s.size() > FP_MAX_ADAPTER_LEN) return false;
+    return true;
+}
+
 bool supported(Options* o, bool hasOverlappedWriter) {
-    return !hasOverlappedWriter && !o->umi.enabled && !o->overRepAnalysis.enabled;
+    return !hasOverlappedWriter && !o->umi.enabled && !o->overRepAnalysis.enabled && adapters_fit(o);
 }
 
 void stage(GpuWorker* w, int side, int64_t i, Read* r) {
@@ -220,6 +232,10 @@ void trace(const char* what, long n) {
     if (g_trace < 0) g_trace = getenv("FASTP_B200_TRACE") ? 1 : 0;
     if (g_trace) fprintf(stderr, "[fastp_b200 binding] %s: %ld units on the device\n", what, n);
 }
+void trace_stock(const char* what, long n) {                                   /* an option set the device path does not cover */
+    if (g_trace < 0) g_trace = getenv("FASTP_B200_TRACE") ? 1 : 0;
+    if (g_trace) fprintf(stderr, "[fastp_b200 binding] %s: %ld units on the stock body\n", what, n);
+}
 
 }  // namespace
 
@@ -228,7 +244,7 @@ bool SingleEndProcessor::processSingleEnd(ReadPack* pack, ThreadConfig* config) 
     int maxLen = 0;
     for (int p = 0; p < pack->count; p++) maxLen = std::max(maxLen, pack->data[p]->length());
     GpuWorker* w = supported(mOptions, false) && maxLen <= FP_MAX_STRIDE ? worker_for(this, mOptions, false, config->getThreadId(), maxLen, pack->count) : nullptr;
-    if (!w) return processSingleEnd_cpu(pack, config);
+    if (!w) { trace_stock("processSingleEnd", pack->count); return processSingleEnd_cpu(pack, config); }
 
     string outstr, failedOut;
     outstr.reserve(pack->count * 320);
@@ -287,7 +303,7 @@ bool PairEndProcessor::processPairEnd(ReadPack* leftPack, ReadPack* rightPack, T
     int maxLen = 0;
     for (int p = 0; p < count; p++) maxLen = std::max(maxLen, std::max(leftPack->data[p]->length(), rightPack->data[p]->length()));
     GpuWorker* w = supported(mOptions, mOverlappedWriter != NULL) && maxLen <= 256 ? worker_for(this, mOptions, true, config->getThreadId(), maxLen, count) : nullptr;
-    if (!w) return processPairEnd_cpu(leftPack, rightPack, config);
+    if (!w) { trace_stock("processPairEnd", count); return processPairEnd_cpu(leftPack, rightPack, config); }
 
     if (leftPack->count != rightPack->count) {                                 /* :363-370 */
         cerr << endl;
